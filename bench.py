@@ -4,11 +4,12 @@
   python bench.py --gpus N --steps K --warmup W                      # this repo's CUDA path, BASELINE configs[1]
   python bench.py --config 3|4|5 [--scaling strong] ...              # the other BASELINE configs (see CONFIGS)
   python bench.py --impl reference --gpus N --steps K ...            # the reference's CPU path on the host cores
+  python bench.py ... --dump-outputs DIR                             # + DIR/sample.npy (sample_rank<r>.npy with several ranks): the last timed sample
 
 One bench "step" = one full sampling call of the workload on every rank (config 2: SMPL diffusion, 100 DDPM steps,
 B=64, T=30, inpainted past of 10 frames); the metric counts the DENOISING steps executed.
 
-  scaling "weak"   (default; the driver's 1/2/4/8 run): every rank samples its own batch of B sequences, no data-path
+  scaling "weak"   (default): every rank samples its own batch of B sequences, no data-path
                    collective (SURVEY 8e);  value = N_ranks * K * n_steps / max-over-ranks time
   scaling "strong" (--scaling strong, and always for configs 4 / 5): ONE global batch sliced into contiguous B/G
                    samples per rank, noise keyed by the global sample index (rank outputs concatenate to the 1-GPU
@@ -47,25 +48,17 @@ CONFIGS = {
                  "global B=128 sharded over the GPUs, T=30 (BASELINE configs[4])", B=128, T=30, past=10, steps=100, correction=True,
             windows=11, strong=True),
 }
-# dram__bytes_read.sum + dram__bytes_write.sum of ONE mlp_fused_kernel launch (ncu --set full, cold caches:
-# profiles/r1_ncu_full_mlp.txt)
-MLP_DRAM_TRAFFIC_BYTES = 6072576
 METRIC = "HOI denoising-steps/sec (B=64,T=30)"
 UNIT = "denoising steps/s"
 
 
 def _peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            d = json.load(f)
-        return dict(hbm_gbs=d["hbm_gbs"], bf16_tflops=d["bf16_tflops"], bf16_tflops_sustained=d.get("bf16_tflops_sustained"),
-                    source="MEASURED_PEAKS.json")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    """data-sheet figures of the H100 SXM at 700 W (dense fp16 / bf16, HBM3): ceilings, not rates this project reached"""
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, source="NVIDIA H100 SXM data sheet")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -114,10 +107,8 @@ def workload_config(cfg_id, scaling, world):
 # CPU arm: the reference's own classes when its tree is reachable, else the oracle port
 # ------------------------------------------------------------------------------------------------------------------
 def _reference_tree():
-    for cand in (os.environ.get("INTERDIFF_REF"), os.path.join(ROOT, "baseline", "_ref"), "/root/reference"):
-        if cand and os.path.isdir(os.path.join(cand, "interdiff", "model")):
-            return cand
-    return None
+    cand = os.environ.get("INTERDIFF_REF")
+    return cand if cand and os.path.isdir(os.path.join(cand, "interdiff", "model")) else None
 
 
 def cpu_reference_rate(cfg_id, n_plain, threads=None, seed=233):
@@ -284,7 +275,7 @@ def run_ours(args):
     if c["correction"]:
         eng.bind_correction(b["hand_pose"], b["betas"], b["obj_points"], past_len=c["past"])
     tape_d = draw_tape_indexed(eng, shape[1:], n, ids, seed=233)              # noise keyed by the GLOBAL sample index
-    flush = torch.empty(256 * 1024 * 1024 // 4, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, device=dev)  # > 50 MB L2
     out = torch.empty(shape, device=dev)
     rollout = None
     if c["windows"] > 1:
@@ -320,6 +311,9 @@ def run_ours(args):
     wall = time.perf_counter() - wall0
     launches = eng.launch_count - l0
     dev_ms = sum(s.elapsed_time(e) for s, e in ev)
+    if args.dump_outputs:       # what the last timed call returned: the sample (B, 1, C, T) of this rank
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "sample.npy" if world == 1 else "sample_rank%d.npy" % rank), out.cpu().numpy().astype(np.float32))
     # ---- end-to-end leg through the public API with host buffers
     pin = lambda a: torch.from_numpy(np.ascontiguousarray(a)).pin_memory()
     h_gt, h_mask, h_cond, h_xT = pin(b["gt"]), pin(b["mask"]), pin(b["cond"]), pin(S.noise_tape(shape, 0, 233 + rank)[0])
@@ -392,10 +386,10 @@ def run_ours(args):
         value = total_steps / (dev_ms / 1000.0)
         line = dict(metric=METRIC, value=value, unit=UNIT, n_gpus=world, steps=args.steps, warmup=max(3, args.warmup),
                     ms_per_step=dev_ms / args.steps, higher_is_better=True, scaling="strong" if strong else "weak", vs_baseline=None,
-                    dtype="f32 (fp32 SIMT GEMMs)" if args.backend == "simt" else "f32-grade (GEMMs: fp16 hi/lo split pairs on tcgen05, fp32 TMEM accumulate; rest fp32)",
+                    dtype="f32 (fp32 SIMT GEMMs)" if args.backend == "simt" else "f32-grade (GEMMs: fp16 hi/lo split pairs on wgmma, fp32 accumulate; rest fp32)",
                     data="synthetic", config=workload_config(args.config, args.scaling, world),
                     run=dict(l2="flushed between timed iterations (256 MB fill outside the event pair)", cuda_graph="whole loop as one graph",
-                             gemm_backend=args.backend or "tcgen05", batch_per_gpu=Bl, us_per_denoising_step=1000.0 * dev_ms / args.steps / per_call,
+                             gemm_backend="fp32 SIMT" if args.backend == "simt" else "wgmma split-fp16 (option name \"tcgen05\")", batch_per_gpu=Bl, us_per_denoising_step=1000.0 * dev_ms / args.steps / per_call,
                              sample_steps_per_s=value * (c["B"] if strong else Bl),
                              body_model="synthetic SMPL-H-shaped model, <= 4 non-zero skinning weights per vertex" if c["correction"] else None),
                     gpu_launches=int(launches), clocks=clocks, wall_s=wall)
@@ -412,19 +406,17 @@ def run_ours(args):
         if roof and roof["ms"] > 0:
             ach = roof["flops"] / (roof["ms"] * 1e-3) / 1e12
             line["roofline"] = dict(bound="tensor", kernel=roof["kernel"], achieved=ach, peak=peaks["bf16_tflops"], unit="TFLOP/s",
-                                    frac=ach / peaks["bf16_tflops"], traffic=MLP_DRAM_TRAFFIC_BYTES, us_per_launch=roof["ms"] * 1e3,
-                                    peak_source=peaks["source"] + " (burst bf16)",
+                                    frac=ach / peaks["bf16_tflops"], us_per_launch=roof["ms"] * 1e3,
+                                    peak_source=peaks["source"] + " (dense fp16 / bf16)",
                                     issue_ceiling=peaks["bf16_tflops"] / 3.0, frac_of_issue_ceiling=ach / (peaks["bf16_tflops"] / 3.0),
                                     note="algorithmic flops 2*M*(256*1024 + 1024*256) = %.3f GFLOP per launch / mean time of %d back-to-back "
                                          "launches (CUDA events); the split-precision kernel issues 3 fp16 MMAs per algorithmic MAC, so its "
-                                         "ceiling is 1/3 of the fp16/bf16 peak; at M=%d the launch is one wave of %d CTAs bound by "
-                                         "fixed latencies (DESIGN.md 4.1b timeline), not by the tensor pipe; traffic = dram bytes per "
-                                         "launch from the ncu --set full capture in profiles/ (operands are L2 resident in the loop)"
+                                         "ceiling is 1/3 of the fp16/bf16 peak; at M=%d the launch is one wave of %d CTAs"
                                          % (roof["flops"] / 1e9, roof["iters"], M, 8 * ((M + 127) // 128)))
         if lbs:
             gbs = lbs["bytes"] / (lbs["ms"] * 1e-3) / 1e9
             tf = lbs["flops"] / (lbs["ms"] * 1e-3) / 1e12
-            line["roofline_lbs"] = dict(bound="hbm", kernel="SMPL-H LBS (k_lbs_pose + tcgen05 blend GEMM + k_lbs_skin_sparse), F=%d frames" % lbs["F"],
+            line["roofline_lbs"] = dict(bound="hbm", kernel="SMPL-H LBS (k_lbs_pose + wgmma blend GEMM + k_lbs_skin_sparse), F=%d frames" % lbs["F"],
                                         achieved=gbs, peak=peaks["hbm_gbs"], unit="GB/s", frac=gbs / peaks["hbm_gbs"], ms=lbs["ms"],
                                         algorithmic_bytes=lbs["bytes"], tflops=tf, tflops_frac_of_bf16_peak=tf / peaks["bf16_tflops"],
                                         note="algorithmic bytes = constants once (41.7 MB) + 84.0 KB per frame (SURVEY 8d); 33.2 MFLOP per frame; "
@@ -450,7 +442,10 @@ def main():
     ap.add_argument("--backend", default=None, choices=[None, "simt", "tcgen05"])
     ap.add_argument("--cpu-steps", type=int, default=6)
     ap.add_argument("--no-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's sample to DIR/sample.npy (float32)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs applies to the CUDA path (--impl ours) only")
     if args.impl == "reference":
         run_reference(args)
     else:

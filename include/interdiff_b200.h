@@ -1,4 +1,4 @@
-/* interdiff_b200.h -- C ABI of libinterdiff_b200.so (sm_100a).
+/* interdiff_b200.h -- C ABI of libinterdiff_b200.so (sm_90a).
  *
  * Drop-in boundary for the InterDiff sampling hot path (SURVEY.md section 8b).  The reference
  * reaches this path through Python module APIs, not an FFI; each entry point below names the
@@ -29,7 +29,7 @@ int idb_create(idb_handle** out);                 /* on the current CUDA device 
 int idb_destroy(idb_handle* h);
 const char* idb_last_error(const idb_handle* h);
 long long idb_launch_count(const idb_handle* h);  /* kernels launched so far through h */
-int idb_set_gemm_backend(idb_handle* h, int backend); /* 0 = fp32 SIMT (debug/bisect), 1 = tcgen05 split-fp16 (default) */
+int idb_set_gemm_backend(idb_handle* h, int backend); /* 0 = fp32 SIMT (debug/bisect), 1 = wgmma split-fp16 (default) */
 /* Programmatic dependent launch between the kernels of a sampling step (default 1). Results are identical
    either way; 0 serialises the kernels (for bisecting / profiling). */
 int idb_set_dependent_launch(idb_handle* h, int on);
@@ -88,7 +88,7 @@ int idb_encode_condition(idb_handle* h, int B, int Tp, const float* past, const 
 
 /* PointNet++ (MSG) point-cloud encoder = MDM.pcEmbedding, PointNet2Encoder(c_in=1, c_out=256, num_keypoints=1)
  * (reference model/layers.py:111-175, called at model/diffusion_smpl.py:210-211); the furthest-point-sampling /
- * ball-query / grouping operators of the un-vendored pointnet2_ops 3.0.0 are rebuilt for sm_100a.
+ * ball-query / grouping operators of the un-vendored pointnet2_ops 3.0.0 are rebuilt for sm_90a.
  * Needs the "pcEmbedding.*" tensors (incl. the BatchNorm running statistics) loaded before idb_denoiser_commit.
  *   obj_points   (B,P,3)   object point cloud in the canonical frame (P = 2048 in the reference; 512..4096)
  *   pc_embedding (B,256)   = pcEmbedding(cat([p, |p|]).unsqueeze(0)).view(1,B,-1)[0]  -> idb_encode_condition */
@@ -221,7 +221,7 @@ int idb_debug_gemm(idb_handle* h, const float* A, const float* W, const float* b
 int idb_debug_gemm_repeat(idb_handle* h, const float* A, const float* W, const float* bias, const float* res, float* C,
                           int M, int N, int K, int epi, int iters, void* stream);
 
-/* test hook: number of round-robin TMEM accumulators of the tcgen05 GEMM (0 = default) */
+/* test hook: k-blocks the wgmma GEMM accumulates in the tensor core between fp32 promotions (0 = default) */
 int idb_debug_set_gemm_accumulators(int n);
 /* out[M][256] = [LayerNorm(] gelu(x w1^T + b1) w2^T + b2 + res [)] through the fused feed-forward kernel (fp32 device
    pointers; ln_w / ln_b NULL = no norm); iters > 1: launches 2..iters are timed (idb_debug_last_ms); trace != NULL:
@@ -235,7 +235,7 @@ int idb_debug_attn_trace(long long* out16);
 /* chain timeline probe (profiles/chain_probe.py): device buffer of 64 lanes x (2 + 2 * capacity) uint64, lane[0] = 0, lane[1] = capacity; every
    kernel of the sampling step then appends (kind | event | grid | block, %globaltimer) records; NULL switches it off */
 int idb_debug_chain_trace(idb_handle* h, unsigned long long* buf);
-/* one launch with a per-CTA clock64 timeline (16 slots per CTA) of the tcgen05 kernel's pipeline */
+/* one launch with a per-CTA clock64 timeline (16 slots per CTA) of the wgmma kernel's pipeline */
 int idb_debug_gemm_trace(idb_handle* h, const float* A, const float* W, float* C, int M, int N, int K, long long* trace, void* stream);
 
 /* debug: fp16 (hi, lo) operand split (x = hi + lo * 2^-11), and a GEMM on such pairs */

@@ -1,7 +1,7 @@
 """ctypes binding of libinterdiff_b200.so (the C ABI in include/interdiff_b200.h).
 
 There is NO CPU or PyTorch fallback: importing the product ops without the built library, or
-calling them without a Blackwell GPU, raises.
+calling them without a Hopper GPU, raises.
 """
 import ctypes as C
 import os

@@ -1,4 +1,4 @@
-"""Build libinterdiff_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Build libinterdiff_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
 import os
 import subprocess
 import sys
@@ -6,8 +6,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libinterdiff_b200.so")
-SOURCES = ["api.cu", "gemm.cu", "gemm_tcgen05.cu", "denoiser.cu", "sampler.cu", "lbs.cu", "geometry.cu", "correction.cu", "pointnet.cu", "metrics.cu", "rollout.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+SOURCES = ["api.cu", "gemm.cu", "gemm_wgmma.cu", "denoiser.cu", "sampler.cu", "lbs.cu", "geometry.cu", "correction.cu", "pointnet.cu", "metrics.cu", "rollout.cu"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 
 
@@ -43,7 +43,7 @@ def build(force=False, verbose=False):
         sys.stderr.write("\n".join(log))
     if failed:
         raise RuntimeError("nvcc failed; see interdiff_b200/build/nvcc.log")
-    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"]
     subprocess.check_call(cmd)
     return LIB
 
@@ -56,7 +56,7 @@ def build_tools():
         return out
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     os.makedirs(os.path.join(HERE, "build"), exist_ok=True)
-    subprocess.check_call([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-o", out, src])
+    subprocess.check_call([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-o", out, src])
     return out
 
 

@@ -20,9 +20,9 @@ extern "C" int idb_create(idb_handle** out) {
     idb_handle* h = new idb_handle();
     h->device = dev;
     h->sm_count = prop.multiProcessorCount;
-    if (prop.major != 10) {
-        // sm_100a-only library: refuse loudly rather than fall back
-        h->err = "interdiff_b200 needs a Blackwell (sm_100) device";
+    if (prop.major != 9) {
+        // sm_90a-only library: refuse loudly rather than fall back
+        h->err = "interdiff_b200 needs a Hopper (sm_90) device";
         *out = h;
         return IDB_ERR_CUDA;
     }
@@ -111,7 +111,7 @@ extern "C" int idb_debug_mlp(idb_handle* h, const float* x, const float* w1, con
     for (int i = 0; i < (iters > 0 ? iters : 1) && !rc; i++) {
         if (i == 0 && trace) g_idb_gemm_trace = trace;
         if (i == 1) cudaEventRecord(e0, st);
-        rc = idb_mlp_tcgen05(h, xh, xl, w1h, w1l, b1, w2h, w2l, b2, res, Dm, out, Dm, M, 0, st, ln_w, ln_b, nullptr, nullptr);
+        rc = idb_mlp_wgmma(h, xh, xl, w1h, w1l, b1, w2h, w2l, b2, res, Dm, out, Dm, M, 0, st, ln_w, ln_b, nullptr, nullptr);
     }
     cudaEventRecord(e1, st);
     cudaStreamSynchronize(st);
@@ -166,13 +166,13 @@ extern "C" int idb_debug_gemm_trace(idb_handle* h, const float* A, const float* 
     return idb_gemm(h, A, K, W, K, nullptr, nullptr, N, C, N, M, N, K, g_idb_trace_epi, (cudaStream_t)stream);
 }
 
-extern int g_idb_gemm_nacc;
-extern int g_idb_gemm_bn192;
-/* test hook: number of round-robin TMEM accumulators for the big x big products (0 = default); 900 / 901: 192-column tiles off / on */
+extern int g_idb_gemm_promote;
+extern int g_idb_gemm_wide_tiles;
+/* test hook: k-blocks the big x big products accumulate in the tensor core between fp32 promotions (0 = default); 900 / 901: 128-column tiles off / on */
 extern "C" int idb_debug_set_gemm_accumulators(int n) {
-    if (n == 900 || n == 901) { g_idb_gemm_bn192 = n - 900; return IDB_OK; }
+    if (n == 900 || n == 901) { g_idb_gemm_wide_tiles = n - 900; return IDB_OK; }
     if (n >= 1000) { g_idb_trace_epi = n - 1000; return IDB_OK; }   // >= 1000: epi flags for idb_debug_gemm_trace
-    g_idb_gemm_nacc = n;
+    g_idb_gemm_promote = n;
     return IDB_OK;
 }
 

@@ -1,4 +1,4 @@
-// Shared internals of libinterdiff_b200.so (sm_100a only).
+// Shared internals of libinterdiff_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -104,10 +104,10 @@ struct Sampler;       // sampler.cu
 
 struct idb_handle {
     std::string err;
-    int device = 0, sm_count = 148;
+    int device = 0, sm_count = 132;
     long long epoch = 0;      // bumped whenever a buffer / table / launch attribute that captured graphs reference changes
     long long launches = 0;   // kernels launched through this handle (bench's gpu_launches)
-    int gemm_backend = 1;     // 0 = fp32 SIMT (debug / bisect), 1 = tcgen05 split-fp16 (default)
+    int gemm_backend = 1;     // 0 = fp32 SIMT (debug / bisect), 1 = wgmma split-fp16 (default)
     int pdl = 1;              // programmatic dependent launch between the kernels of a sampling step
     unsigned attr_mask = 0;   // kernels whose > 48 KB shared-memory opt-in was done on this handle's device (bit 0 GEMM, 1 MLP, 2 NN)
     double last_ms = 0.0;     // mean launch time of the last timed debug hook
@@ -115,9 +115,8 @@ struct idb_handle {
     int nn_pruning = 1;       // cluster-pruned nearest-neighbour search for body-mesh targets (identical results)
     int fuse_attn = 1;        // standard decoder layers: self-attention + cross-attention in one launch (idb_set_fused_mlp(h, 10 / 11) = off / on)
     int fused_mlp = 2;        // feed-forward block as ONE cluster kernel (tensor backend, d_model 256, d_ff 1024); 2 = incl. the layer's final norm;
-                              // 3 = a layer's attention half runs in the same kernel on sample-aligned tiles (one launch per layer):
-                              // measured NOT faster (288.6 vs 282.3 us per step at B=60: programmatic dependent launch already hides the
-                              // boundary) and at B=64 it needs 16 clusters where the device holds 15 (profiles/README.md) - kept as an option
+                              // 3 = a layer's attention half runs in the same kernel on sample-aligned tiles (one launch per layer) -
+                              // an option: programmatic dependent launch already hides most of the boundary
     void* metrics_ws = nullptr; size_t metrics_bytes = 0;        // workspace of idb_metrics (posed object points, normals, signed distances)
     void* scratch = nullptr; size_t scratch_bytes = 0;   // on-the-fly operand splits of idb_gemm
     Denoiser den;
@@ -174,8 +173,8 @@ __device__ __forceinline__ float warp_max(float v) {
 }
 // Exact (erf) GELU, F.gelu default (model/layers.py / nn.TransformerDecoderLayer activation="gelu").
 // erf(t) = 1 - 2^(-t q(t)) with a degree-7 minimax fit of q(t) = -log2(erfc(t)) / t on (0, 4] (erf(4) rounds to
-// 1 in fp32), branch-free: 7 FMA + one MUFU.EX2.  Max abs error of erf 1.0e-7 (libdevice erff: 6e-8; the fit
-// is in profiles/README.md), i.e. fp32-rounding level for the GELU output, at less than half the instructions
+// 1 in fp32), branch-free: 7 FMA + one MUFU.EX2.  Max abs error of erf 1.0e-7 (libdevice erff: 6e-8; checked on a grid
+// by tests/test_gpu_gemm.py), i.e. fp32-rounding level for the GELU output, at less than half the instructions
 // of erff's two-sided evaluation under divergence.
 __device__ __forceinline__ float erf_fast(float x) {
     const float t = fminf(fabsf(x), 4.0f);
@@ -195,53 +194,20 @@ __device__ __forceinline__ float gelu_erf(float x) {
     const float hx = 0.5f * x;
     return fmaf(hx, erf_fast(x * 0.70710678118654752440f), hx);
 }
-// ---- packed fp32 pairs (fma / mul / add .f32x2, sm_100): the same IEEE operations as the scalar code, two per issue slot
-typedef unsigned long long f32x2_t;
-__device__ __forceinline__ f32x2_t pk2(float a, float b) { f32x2_t r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
-__device__ __forceinline__ void upk2(f32x2_t v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ f32x2_t fma2(f32x2_t a, f32x2_t b, f32x2_t c) { f32x2_t d; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c)); return d; }
-__device__ __forceinline__ f32x2_t mul2(f32x2_t a, f32x2_t b) { f32x2_t d; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ f32x2_t add2(f32x2_t a, f32x2_t b) { f32x2_t d; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
 // two elements of the feed-forward block's hidden layer: v = gelu_erf(fmaf(small, 2^-11, main) + bias), returned as the fp16
-// (hi, lo) words of split_f16x2(v0, v1).  Operation for operation the scalar gelu_erf / erf_fast / split_f16x2 (bit-identical),
-// with every fp32 multiply / add / fma issued as a packed pair: the phase is bound by the SM's instruction issue rate.
+// (hi, lo) words of split_f16x2(v0, v1)
 __device__ __forceinline__ void gelu_split_x2(float m0, float m1, float s0, float s1, float2 bias, uint32_t& hi_w, uint32_t& lo_w) {
-    const f32x2_t x = add2(fma2(pk2(s0, s1), pk2(1.0f / 2048.0f, 1.0f / 2048.0f), pk2(m0, m1)), pk2(bias.x, bias.y));
-    const f32x2_t hx = mul2(x, pk2(0.5f, 0.5f));
-    const f32x2_t y = mul2(x, pk2(0.70710678118654752440f, 0.70710678118654752440f));
-    float y0, y1;
-    upk2(y, y0, y1);
-    const float t0 = fminf(fabsf(y0), 4.0f), t1 = fminf(fabsf(y1), 4.0f);
-    const f32x2_t t = pk2(t0, t1);
-    f32x2_t p = pk2(4.5338660129345953e-05f, 4.5338660129345953e-05f);
-    p = fma2(p, t, pk2(-0.0004454450972843915f, -0.0004454450972843915f));
-    p = fma2(p, t, pk2(0.0014896064531058073f, 0.0014896064531058073f));
-    p = fma2(p, t, pk2(0.0007736838888376951f, 0.0007736838888376951f));
-    p = fma2(p, t, pk2(-0.028252195566892624f, -0.028252195566892624f));
-    p = fma2(p, t, pk2(0.1484806090593338f, 0.1484806090593338f));
-    p = fma2(p, t, pk2(0.9184166789054871f, 0.9184166789054871f));
-    p = fma2(p, t, pk2(1.6279085874557495f, 1.6279085874557495f));
-    float a0, a1, e0, e1;
-    upk2(mul2(t, p), a0, a1);          // erf_fast evaluates (-t) * p: the sign moves into the MUFU operand
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(-a0));
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(-a1));
-    float r0, r1;
-    upk2(fma2(pk2(e0, e1), pk2(-1.0f, -1.0f), pk2(1.0f, 1.0f)), r0, r1);      // 1 - e (one rounding, like the scalar subtraction)
-    const f32x2_t v = fma2(hx, pk2(copysignf(r0, y0), copysignf(r1, y1)), hx);
-    float v0, v1;
-    upk2(v, v0, v1);
+    const float v0 = gelu_erf(fmaf(s0, 1.0f / 2048.0f, m0) + bias.x), v1 = gelu_erf(fmaf(s1, 1.0f / 2048.0f, m1) + bias.y);
     const __half2 hh = __floats2half2_rn(v0, v1);
     const float2 f = __half22float2(hh);
-    float l0, l1;
-    upk2(mul2(fma2(pk2(f.x, f.y), pk2(-1.0f, -1.0f), v), pk2(2048.0f, 2048.0f)), l0, l1);      // (v - hi) * 2^11, v - hi exact
-    const __half2 ll = __floats2half2_rn(l0, l1);
+    const __half2 ll = __floats2half2_rn((v0 - f.x) * 2048.0f, (v1 - f.y) * 2048.0f);      // v - hi is exact
     hi_w = *reinterpret_cast<const uint32_t*>(&hh); lo_w = *reinterpret_cast<const uint32_t*>(&ll);
 }
 __device__ __forceinline__ float silu(float x) { return x / (1.0f + expf(-x)); }
 
 // Programmatic dependent launch: every kernel of the sampling step releases its successor at once
 // (pdl_trigger) and blocks (pdl_wait) before its first access to data produced by earlier kernels, so
-// the successor's launch latency, barrier/TMEM setup and constant-weight prefetch overlap the
+// the successor's launch latency, barrier setup and constant-weight prefetch overlap the
 // predecessor's tail.  Both are no-ops for launches without the attribute.  Every kernel in the
 // chain executes pdl_wait, which makes completion transitive along the stream.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -302,13 +268,13 @@ struct GemmArgs {
     int ksplit = 1;                                     // 2: split-K onto a C zeroed by an earlier kernel (tensor path only)
     float* zero = nullptr; int zero_ld = 0, zero_cols = 0;   // aux [M][zero_cols] matrix to clear as a side job
     int pdl = 0;   // 1: programmatic dependent launch; REQUIRES W_hi/W_lo to be complete before the previous kernel started
-    int single_acc = 0;   // 1: ONE main accumulator is accurate enough for the caller whatever K is (e.g. the mm-scale pose
-                          //    blend added to metre-scale vertices): allows the 256-column tiles for long reductions
+    int single_acc = 0;   // 1: ONE tensor-core accumulator is accurate enough for the caller whatever K is (e.g. the mm-scale pose
+                          //    blend added to metre-scale vertices): no fp32 promotion between k-blocks, multicast row-tile pairs
 };
 int idb_gemm_ex(idb_handle* h, const GemmArgs& g, cudaStream_t st);
-// fused feed-forward block on the tensor path (gemm_tcgen05.cu)
-bool idb_mlp_tcgen05_supported(int d_model, int d_ff);
-int idb_mlp_tcgen05(idb_handle* h, const __half* x_hi, const __half* x_lo, const __half* w1_hi, const __half* w1_lo, const float* b1,
+// fused feed-forward block on the tensor path (gemm_wgmma.cu)
+bool idb_mlp_wgmma_supported(int d_model, int d_ff);
+int idb_mlp_wgmma(idb_handle* h, const __half* x_hi, const __half* x_lo, const __half* w1_hi, const __half* w1_lo, const float* b1,
                     const __half* w2_hi, const __half* w2_lo, const float* b2, const float* res, int ldr, float* Z, int ldz, int M,
                     int pdl, cudaStream_t st, const float* ln_w = nullptr, const float* ln_b = nullptr, __half* Z_hi = nullptr,
                     __half* Z_lo = nullptr);

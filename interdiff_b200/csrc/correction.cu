@@ -664,7 +664,7 @@ int idb_correction_apply_dev(idb_handle* h, float* x0, const float* gt, int t, c
     if ((rc = projector_run(h, T, B, p.gt_ang, p.gt_tr, p.markers, p.contact, p.proj_out, st))) return rc;
     // t[0] / 1000 in float32 (torch true-divides the int64 tensor by 1000 -> float32)
     const float a = (float)t / 1000.0f;
-    k_blend<<<148 * 2, 256, 0, st>>>(x0, p.proj_out, p.cond, a, B, T, C);
+    k_blend<<<132 * 2, 256, 0, st>>>(x0, p.proj_out, p.cond, a, B, T, C);
     LAUNCH_CHECK(h);
     return IDB_OK;
 }

@@ -215,14 +215,11 @@ constexpr uint32_t ROW_BYTES = D * sizeof(float);
 
 // --- 16-row tensor-core fragments.  The three small products of the fused QaN / cross-attention kernel
 // ([18 x 256] x [256 x 30], [16 x 256] x [256 x 40], [16 x 40] x [40 x 256]) are far too small for a
-// tcgen05 tile (M = 128) but are exactly one mma.sync m16n8k16 row block.  fp32 operands are read from
+// wgmma tile (M = 64) but are exactly one mma.sync m16n8k16 row block.  fp32 operands are read from
 // shared memory straight into fragments (row strides of 8 mod 32 floats for the float2 k-pairs, 4 mod 16
 // for the K x N values, make every fragment load conflict-free), split on the fly into the same fp16
 // (hi, lo * 2^11) pairs as the big GEMMs and multiplied as hi*hi (main accumulator) and lo*hi + hi*lo
 // (small accumulator, folded in with 2^-11): fp32-grade, ~3e-7 over K = 256 with the 4-way k-split.
-// History (profiles/README.md): the register-tiled SIMT version was bound by shared-memory wavefronts
-// (4-way replays of its 128-bit operand loads); a 3xTF32 m16n8k8 version was no faster because legacy
-// TF32 mma.sync issues at ~30 cycles per instruction and scheduler on this part (= the FFMA rate).
 constexpr int LDX = D + 8;     // row stride of fragment-A / row-dot operands (x rows, folded queries / keys): 8 mod 32
 constexpr int VLD = D + 4;     // row stride of the folded values (K x N fragments): 4 mod 16
 constexpr int PLD = 72;        // row stride of the probabilities: 8 mod 32
@@ -631,7 +628,7 @@ k_xattn_ln(const XattnArgs xa) {
 
 // Standard decoder layer, attention half in ONE launch: self-attention + LN1 (attn_body) and - on the rows this CTA has just
 // written - cross-attention + LN2 (xattn_body), on the same shared memory one after the other.  Saves the kernel boundary
-// between the two (hand-off, CTA launch, a second prologue: ~3 us of a step's critical path per layer).
+// between the two (hand-off, CTA launch, a second prologue).
 __global__ void __launch_bounds__(ANT)
 k_attn_xattn_ln(const AttnArgs aa, const XattnArgs xa) {
     extern __shared__ __align__(16) float sm[];
@@ -850,7 +847,7 @@ k_qan_xattn_ln(const QanArgs qa) {
 // cluster barrier the same 8 CTAs run the feed-forward block on the cluster's rows as one 128-row tile (rows past G T belong to
 // the next cluster: computed, never reduced or stored).  Tiles aligned to samples mean NO dependency between clusters, so the
 // kernel boundary between the two halves of a layer disappears.  The attention phase uses the operand region of the
-// feed-forward block as its shared memory; the feed-forward barriers and the TMEM allocation sit above it and are set up at entry.
+// feed-forward block as its shared memory; the feed-forward barriers sit above it and are set up at entry.
 __global__ void __cluster_dims__(tc::mlp::CLUSTER, 1, 1) __launch_bounds__(ANT, 1)
 k_layer_qan_fused(const QanArgs qa, const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w1,
                   const __grid_constant__ CUtensorMap map_xl, const __grid_constant__ CUtensorMap map_w1l,
@@ -862,7 +859,7 @@ k_layer_qan_fused(const QanArgs qa, const __grid_constant__ CUtensorMap map_x, c
     pdl_trigger();
     const int c = blockIdx.x, cl = blockIdx.y, tid = threadIdx.x;
     tc::MlpArgs a{&map_x, &map_w1, &map_xl, &map_w1l, &map_w2, &map_w2l, b1, b2, res, D, Z, D, ln_w, ln_b, Zh, Zl, nullptr};
-    const uint32_t tmem_base = tc::mlp_setup<8>(smem_raw, a);
+    tc::mlp_setup(smem_raw, a);
     // ---- phase A
     const int sl = c / nslabs, b = cl * G + sl;
     const bool attend = sl < G && b < qa.B;
@@ -880,8 +877,7 @@ k_layer_qan_fused(const QanArgs qa, const __grid_constant__ CUtensorMap map_x, c
     asm volatile("fence.proxy.async;" ::: "memory");
     // ---- phase B
     const int m0 = cl * G * qa.T;
-    tc::mlp_run<8>(smem_raw, a, c, m0, min(M, m0 + G * qa.T), tmem_base, false, nullptr);
-    tc::mlp_teardown(tmem_base);
+    tc::mlp_run(smem_raw, a, c, m0, min(M, m0 + G * qa.T), false, nullptr);
 }
 
 // The same for a standard decoder layer (layers 0 and 7): self-attention + LN1 (phase A1, on the folded-QKV projection a
@@ -897,7 +893,7 @@ k_layer_std_fused(const AttnArgs aa, const XattnArgs xa, const __grid_constant__
     pdl_trigger();
     const int c = blockIdx.x, cl = blockIdx.y, tid = threadIdx.x;
     tc::MlpArgs a{&map_x, &map_w1, &map_xl, &map_w1l, &map_w2, &map_w2l, b1, b2, res, D, Z, D, ln_w, ln_b, Zh, Zl, nullptr};
-    const uint32_t tmem_base = tc::mlp_setup<8>(smem_raw, a);
+    tc::mlp_setup(smem_raw, a);
     const int sl = c / nslabs, b = cl * G + sl, r0 = (c % nslabs) * SLAB;
     const bool attend = sl < G && b < xa.B;
     float* sm = reinterpret_cast<float*>(smem_raw);
@@ -923,8 +919,7 @@ k_layer_std_fused(const AttnArgs aa, const XattnArgs xa, const __grid_constant__
     tc::cluster_sync_all();
     asm volatile("fence.proxy.async;" ::: "memory");
     const int m0 = cl * G * xa.T;
-    tc::mlp_run<8>(smem_raw, a, c, m0, min(M, m0 + G * xa.T), tmem_base, false, nullptr);
-    tc::mlp_teardown(tmem_base);
+    tc::mlp_run(smem_raw, a, c, m0, min(M, m0 + G * xa.T), false, nullptr);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1163,7 +1158,7 @@ extern "C" int idb_debug_attn_trace(long long* out16) {
 // ------------------------------------------------------------------------------------------
 
 int idb_pointnet_commit(idb_handle* h);
-// six tensor maps of the feed-forward block (x hi/lo rows [M][256], w1 hi/lo [1024][256], w2 hi/lo [256][1024]); gemm_tcgen05.cu
+// six tensor maps of the feed-forward block (x hi/lo rows [M][256], w1 hi/lo [1024][256], w2 hi/lo [256][1024]); gemm_wgmma.cu
 int idb_mlp_make_maps(idb_handle* h, const __half* x_hi, const __half* x_lo, const __half* w1_hi, const __half* w1_lo, const __half* w2_hi,
                       const __half* w2_lo, int M, CUtensorMap* out6);
 void idb_pointnet_release(idb_handle* h);
@@ -1608,7 +1603,7 @@ static int denoiser_layers(idb_handle* h, cudaStream_t st) {
     const int ln_blocks = (M * 32 + 255) / 256;
     const DenoiserLayer* pending = nullptr;   // layer whose norm3 has not been applied to d.z yet (unfused feed-forward path)
     const bool pdl = h->pdl != 0;
-    const bool fused = h->gemm_backend == 1 && h->fused_mlp && idb_mlp_tcgen05_supported(D, F);
+    const bool fused = h->gemm_backend == 1 && h->fused_mlp && idb_mlp_wgmma_supported(D, F);
     int rc;
     for (auto& L : d.layers) {
         // ---- first sub-block -> x1 = (d.h2, h2_b, h2_s)
@@ -1677,12 +1672,12 @@ static int denoiser_layers(idb_handle* h, cudaStream_t st) {
             // both GEMMs, GELU, the residual AND the layer's norm3 in one cluster kernel: the hidden activations never
             // leave the SM and the next layer starts from normalised rows (fp32 + fp16 pairs)
             if (h->fused_mlp >= 2) {
-                if ((rc = idb_mlp_tcgen05(h, d.h2_b, d.h2_s, L.w1_b, L.w1_s, L.b1, L.w2_b, L.w2_s, L.b2, d.h2, D, d.h, D, M, h->pdl, st,
+                if ((rc = idb_mlp_wgmma(h, d.h2_b, d.h2_s, L.w1_b, L.w1_s, L.b1, L.w2_b, L.w2_s, L.b2, d.h2, D, d.h, D, M, h->pdl, st,
                                           L.ln3w, L.ln3b, d.h_b, d.h_s)))
                     return rc;
                 continue;
             }
-            if ((rc = idb_mlp_tcgen05(h, d.h2_b, d.h2_s, L.w1_b, L.w1_s, L.b1, L.w2_b, L.w2_s, L.b2, d.h2, D, d.z, D, M, h->pdl, st)))
+            if ((rc = idb_mlp_wgmma(h, d.h2_b, d.h2_s, L.w1_b, L.w1_s, L.b1, L.w2_b, L.w2_s, L.b2, d.h2, D, d.z, D, M, h->pdl, st)))
                 return rc;
         } else {
             // ff1 also clears d.z (dead here) so that ff2 can run split-K = 2 and fill 120 SMs instead of 60
@@ -1860,7 +1855,7 @@ extern "C" int idb_encode_condition(idb_handle* h, int B, int Tp, const float* p
     const int M = B * Tp, F = c.d_ff, H = c.n_heads, N = c.n_queries, C = c.c_body + c.c_obj, Cp = (C + 7) & ~7;
     if (c.variant != 0) return idb_fail(h, IDB_ERR_ARG, "idb_encode_condition: SMPL model only");
     cudaStream_t st = (cudaStream_t)stream;
-    const bool fused = h->gemm_backend == 1 && h->fused_mlp && idb_mlp_tcgen05_supported(D, F);
+    const bool fused = h->gemm_backend == 1 && h->fused_mlp && idb_mlp_wgmma_supported(D, F);
     if (M > d.enc_cap) {
         for (void* p : d.enc_owned) cudaFree(p);
         d.enc_owned.clear();
@@ -1909,12 +1904,12 @@ extern "C" int idb_encode_condition(idb_handle* h, int B, int Tp, const float* p
         }
         if (fused) {
             if (h->fused_mlp >= 2) {
-                if ((rc = idb_mlp_tcgen05(h, d.e_h2_b, d.e_h2_s, L.w1_b, L.w1_s, L.b1, L.w2_b, L.w2_s, L.b2, d.e_h2, D, d.e_h, D, M, h->pdl,
+                if ((rc = idb_mlp_wgmma(h, d.e_h2_b, d.e_h2_s, L.w1_b, L.w1_s, L.b1, L.w2_b, L.w2_s, L.b2, d.e_h2, D, d.e_h, D, M, h->pdl,
                                           st, L.ln3w, L.ln3b, d.e_h_b, d.e_h_s)))
                     return rc;
                 continue;
             }
-            if ((rc = idb_mlp_tcgen05(h, d.e_h2_b, d.e_h2_s, L.w1_b, L.w1_s, L.b1, L.w2_b, L.w2_s, L.b2, d.e_h2, D, d.e_z, D, M, h->pdl, st)))
+            if ((rc = idb_mlp_wgmma(h, d.e_h2_b, d.e_h2_s, L.w1_b, L.w1_s, L.b1, L.w2_b, L.w2_s, L.b2, d.e_h2, D, d.e_z, D, M, h->pdl, st)))
                 return rc;
         } else {
             if ((rc = linear(h, d.e_h2_b, d.e_h2_s, D, L.w1_b, L.w1_s, D, L.b1, nullptr, nullptr, d.e_ff_b, d.e_ff_s, F, M, F, D,

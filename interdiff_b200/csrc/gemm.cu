@@ -4,11 +4,11 @@
 // plain TF32/FP16/BF16 operand rounding diverges to O(1) over a 100-1000 step loop):
 //   backend 0: fp32 SIMT register-tiled kernel (this file) -- debug / bisect path and fallback
 //              for shapes the tensor-core kernel does not take.
-//   backend 1: tcgen05 split-precision kernel on fp16 (hi, lo) operand pairs (gemm_tcgen05.cu), default.
+//   backend 1: wgmma split-precision kernel on fp16 (hi, lo) operand pairs (gemm_wgmma.cu), default.
 #include "common.cuh"
 
-int idb_gemm_tcgen05(idb_handle* h, const GemmArgs& g, cudaStream_t st);
-bool idb_gemm_tcgen05_supported(const GemmArgs& g);
+int idb_gemm_wgmma(idb_handle* h, const GemmArgs& g, cudaStream_t st);
+bool idb_gemm_wgmma_supported(const GemmArgs& g);
 
 namespace {
 
@@ -184,7 +184,7 @@ int idb_gemm_ex(idb_handle* h, const GemmArgs& g_in, cudaStream_t st) {
             g.W_hi = hi; g.W_lo = lo; g.ldw = Kp;
             g.pdl = 0;   // the weight pairs were produced just now on this stream: no early tile fetch
         }
-        if (idb_gemm_tcgen05_supported(g)) return idb_gemm_tcgen05(h, g, st);
+        if (idb_gemm_wgmma_supported(g)) return idb_gemm_wgmma(h, g, st);
     }
     // fp32 SIMT path (prefers the full-precision operand when both forms are available); full K, plain
     // stores, so only the aux-zero side job of the tensor path has to be reproduced

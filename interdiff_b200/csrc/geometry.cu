@@ -142,7 +142,7 @@ k_signed_nn_pruned(const float* __restrict__ query, const float* __restrict__ ta
         // bound (2e-4 relative slack on the safe side, inclusive so that ties are visited); (3) the candidates are walked in
         // id order, each re-tested against the CURRENT warp-uniform bound (one shuffle for its lower bound, one redux.min on
         // the distance bits after every scan), so clusters that stopped mattering are skipped for 4 instructions.  (A strict
-        // best-first order was measured slower: 6.7 vs 4.3 ms, its per-step arg-min costs more than the scans it saves.)
+        // best-first order costs a per-step arg-min that outweighs the scans it saves.)
         float lb2[NN_CLUSTERS / 32];
         unsigned key = 0xffffffffu;
 #pragma unroll

@@ -184,8 +184,8 @@ k_lbs_skin(const float* __restrict__ posedirsT, const float* __restrict__ shaped
 
 
 // Second half of the tensor-core path.  The pose blend  P vec(R - I)  and the shape blend  S beta  (the 469 multiply-adds per
-// vertex coordinate) are ONE split-precision tcgen05 GEMM  blend[F][3V] = [pose_map | beta][F][469] . (2^8 [P | S])[3V][469]^T
-// (gemm_tcgen05.cu; fp16 (hi, lo) pairs, fp32 TMEM accumulation; the 2^8 keeps the mm-scale bases well inside the fp16 normal
+// vertex coordinate) are ONE split-precision wgmma GEMM  blend[F][3V] = [pose_map | beta][F][469] . (2^8 [P | S])[3V][469]^T
+// (gemm_wgmma.cu; fp16 (hi, lo) pairs, fp32 register accumulation; the 2^8 keeps the mm-scale bases well inside the fp16 normal
 // range and is undone exactly below; the metre-scale template stays out of the tensor core's truncating accumulation).
 // This kernel finishes a vertex: template + blend, skinning matrix from the
 // vertex's non-zero bones only (SMPL weights have <= 4 per vertex; ELL list built at init, dense walk as the fallback),
@@ -469,7 +469,7 @@ extern "C" int idb_smplh_lbs(idb_handle* h, int F, const float* pose, const floa
     int rc = idb_body_workspace(h, F);
     if (rc) return rc;
     const size_t smem_pose = sizeof(float) * (size_t)m.J * (9 + 3 + 12);
-    // tensor backend: the 459-term pose blend is a split-precision tcgen05 GEMM, the rest a sparse-bone skinning kernel
+    // tensor backend: the 459-term pose blend is a split-precision wgmma GEMM, the rest a sparse-bone skinning kernel
     const bool tensor = h->gemm_backend == 1 && verts && m.pd_hi;
     k_lbs_pose<<<F, 64, smem_pose, st>>>(pose, betas, trans, m.J_templ, m.J_shape, m.parents, m.A, m.pose_map, jtr, m.J, m.NB, m.Kp,
                                          tensor ? m.pm_hi : nullptr, tensor ? m.pm_lo : nullptr, m.Kld, m.depth, m.max_depth);

@@ -4,7 +4,7 @@
 //
 // The reference delegates the point operators to the un-vendored CUDA extension pointnet2_ops 3.0.0
 // (furthest_point_sampling, ball_query, group_points; generic SIMT code whose arch list stops at sm_75).
-// They are rebuilt here for sm_100a following that version's published algorithm - the same statement the
+// They are rebuilt here for sm_90a following that version's published algorithm - the same statement the
 // oracle (oracle/pointnet2_restated.py) follows, with the same evaluation order of the float32 distances
 // ((dx*dx + dy*dy) + dz*dz, no FMA contraction) so that every discrete decision (which point is the
 // furthest, which points are in the ball) is reproduced exactly:

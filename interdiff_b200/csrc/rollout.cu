@@ -78,7 +78,7 @@ extern "C" int idb_add_offset(idb_handle* h, int T, int B, int K, long long ld, 
     IDB_ENTER(h);
     if (!h || !x || !offset || T <= 0 || B <= 0 || K <= 0 || ld < (long long)col0 + 3LL * K) return IDB_ERR_ARG;
     const long long n = (long long)T * B * K * 3;
-    const int blocks = (int)((n + 255) / 256 < 148 * 8 ? (n + 255) / 256 : 148 * 8);
+    const int blocks = (int)((n + 255) / 256 < 132 * 8 ? (n + 255) / 256 : 132 * 8);
     k_add_offset<<<blocks, 256, 0, (cudaStream_t)stream>>>(x, ld, col0, K, T, B, offset, sign);
     LAUNCH_CHECK(h);
     return IDB_OK;

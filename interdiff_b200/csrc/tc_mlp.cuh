@@ -1,5 +1,5 @@
-// tcgen05 / TMA / mbarrier PTX wrappers and the fused feed-forward block as a device function, shared by
-// gemm_tcgen05.cu (stand-alone kernels) and denoiser.cu (the fused decoder-layer kernel).  sm_100a only.
+// wgmma / TMA / mbarrier PTX wrappers and the fused feed-forward block as a device function, shared by
+// gemm_wgmma.cu (stand-alone kernels) and denoiser.cu (the fused decoder-layer kernel).  sm_90a only.
 #pragma once
 #include "common.cuh"
 
@@ -7,16 +7,25 @@
 
 namespace tc {
 
-constexpr int BM = 128;
+constexpr int BM = 128;                // rows per CTA tile: two consumer warpgroups of 64 rows (one wgmma M each)
 constexpr int BK = 64;                 // 64 fp16 = one 128-byte swizzle row
-constexpr int UMMA_K = 16;             // kind::f16
-constexpr int NUM_THREADS = 320;
+constexpr int MMA_K = 16;              // wgmma k per instruction for fp16 operands
+constexpr int NUM_THREADS = 320;       // 8 consumer warps + TMA producer warp + exchange warp
 
 // ---------------------------------------------------------------- PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+// arrive on the barrier at the same offset in CTA `rank` of the cluster
+__device__ __forceinline__ void mbar_arrive_remote(uint32_t bar, uint32_t rank) {
+    uint32_t rbar;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rbar) : "r"(bar), "r"(rank));
+    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(rbar) : "memory");
 }
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
@@ -43,27 +52,7 @@ __device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const CUtensorMap* 
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%4, %5}], [%2], %3;"
                  ::"r"(dst), "l"(map), "r"(bar), "h"(mask), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// the same arrive on the barrier at this offset in every CTA of `mask` (MMA_1SM + TMA multicast: a stage is free when all
-// CTAs that write into it have consumed their copy)
-__device__ __forceinline__ void umma_commit_mc(uint32_t bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask) : "memory");
-}
-// one lane of a fully active warp; the surrounding code stays warp-uniform so that descriptors and
-// addresses live in uniform registers (a divergent `if (lane == 0)` region forces an R2UR per operand)
+// one lane of a fully active warp; the surrounding code stays warp-uniform
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
     asm volatile(
@@ -75,43 +64,91 @@ __device__ __forceinline__ bool elect_one() {
     return pred != 0;
 }
 
-// K-major, SWIZZLE_128B canonical layout: rows of 128 B, 8-row groups 1024 B apart.
+// K-major, SWIZZLE_128B canonical layout: rows of 128 B, 8-row groups 1024 B apart (wgmma matrix descriptor).
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr & 0x3FFFF) >> 4);     // start address  [0,14)
     d |= (uint64_t)1 << 16;                       // leading byte offset (16 B, unused for swizzled K-major)
     d |= (uint64_t)(1024 >> 4) << 32;             // stride byte offset: 8 rows x 128 B
-    d |= (uint64_t)1 << 46;                       // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;                       // SWIZZLE_128B
+    d |= (uint64_t)1 << 62;                       // SWIZZLE_128B
     return d;
+}
+
+// ---- wgmma: D[64 x N] (+)= A[64 x 16] . B[N x 16]^T, fp16 operands read from shared memory through descriptors, fp32
+// accumulators in registers.  Thread (warp w of the warpgroup, lane l) holds, for j = 0 .. N/8 - 1:
+//   d[4j], d[4j+1] = D[16w + l/4][8j + 2(l%4) + {0, 1}],   d[4j+2], d[4j+3] = the same columns of row + 8.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+#define IDB_ACC8(d, i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+__device__ __forceinline__ void wgmma_f16(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, "
+        "%27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t"
+        "}"
+        : IDB_ACC8(d, 0), IDB_ACC8(d, 8), IDB_ACC8(d, 16), IDB_ACC8(d, 24)
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_f16(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, "
+        "%27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, "
+        "%52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t"
+        "}"
+        : IDB_ACC8(d, 0), IDB_ACC8(d, 8), IDB_ACC8(d, 16), IDB_ACC8(d, 24), IDB_ACC8(d, 32), IDB_ACC8(d, 40), IDB_ACC8(d, 48), IDB_ACC8(d, 56)
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+#undef IDB_ACC8
+
+// One k-block (64 columns) of the split-precision product on this warpgroup's 64 rows:
+//   small += A_lo W_hi^T + A_hi W_lo^T,   main (+)= A_hi W_hi^T        (descriptors of the k-block's first 16 columns)
+template <int NR>
+__device__ __forceinline__ void split_kblock(float (&main)[NR], float (&small)[NR], uint64_t dah, uint64_t dal, uint64_t dwh, uint64_t dwl,
+                                             bool first_main, bool first_small, bool with_small = true) {
+#pragma unroll
+    for (int kk = 0; kk < BK / MMA_K; kk++) {
+        const uint64_t koff = (uint64_t)((kk * MMA_K * 2) >> 4);   // +32 bytes per k-step in the start-address field
+        if (with_small) {
+            wgmma_f16(small, dal + koff, dwh + koff, (kk || !first_small) ? 1u : 0u);
+            wgmma_f16(small, dah + koff, dwl + koff, 1u);
+        }
+        wgmma_f16(main, dah + koff, dwh + koff, (kk || !first_main) ? 1u : 0u);
+    }
 }
 
 // ---------------------------------------------------------------------------------------------
 // Fused feed-forward block  Z = gelu(X W1^T + b1) W2^T + b2 + R   for d_model 256, d_ff = 8 x 128.
 //
-// The two GEMMs of a decoder layer are each far below one wave of work (120 / 60 tiles) and their
-// launches, prologues and the 16 MB round trip of the fp16-pair intermediate cost more than the
-// tensor work.  Here a cluster of 8 CTAs owns one 128-row tile: CTA j computes the 128-column chunk j
-// of the hidden layer (GEMM 1, K = 256) into TMEM, its epilogue warps apply bias + GELU, split the
-// result into (hi, lo) fp16 pairs and write them into shared memory directly in the K-major
-// 128B-swizzled layout the tensor core reads (S, one k-block of 64 hidden columns at a time).
+// The two GEMMs of a decoder layer are each below one wave of work and their launches, prologues and the round trip of
+// the fp16-pair intermediate cost more than the tensor work.  Here a cluster of 8 CTAs owns one 128-row tile: CTA j
+// computes the 128-column chunk j of the hidden layer (GEMM 1, K = 256) into the registers of its two consumer
+// warpgroups, which apply bias + GELU, split the result into (hi, lo) fp16 pairs and write them into shared memory
+// directly in the K-major 128B-swizzled layout wgmma reads (S, one k-block of 64 hidden columns at a time).
 //
 // GEMM 2 runs on PAIRS of CTAs (j, j^1): as soon as a k-block of S is complete its owner also copies it into the
-// partner's shared memory (cp.async.bulk shared::cta -> shared::cluster, completing on the partner's mbarrier) - that
-// transfer hides behind the GELU phase - and each CTA of the pair multiplies BOTH hidden chunks (K = 256) with its HALF of
-// the output columns (N = 128, CTA j owns columns 128 (j & 1) ..).  So only 4 instead of 8 partial products exist per
-// output element and each is half as wide: the reduction that ends the kernel - CTA j PULLS rows 16j .. 16j+15 of the
-// partials of both column halves over distributed shared memory and sums them in rank order (deterministic) - moves
-// 56 KB per CTA instead of 112 KB.  That exchange is bound by the SM-to-SM network at ~14 B/clk/SM however it is issued
-// (profiles/dsmem_bench.cu: remote loads, remote stores and bulk copies all land at 13.8 - 14.4 B/clk/SM with 120 CTAs
-// exchanging), so halving the bytes is what shortens it.  Then bias + residual, the layer's final LayerNorm, stores.
+// partner's shared memory (cp.async.bulk shared::cta -> shared::cluster, completing on the partner's mbarrier) and each
+// CTA of the pair multiplies BOTH hidden chunks (K = 256) with its HALF of the output columns (N = 128, CTA j owns
+// columns 128 (j & 1) ..).  So only 4 instead of 8 partial products exist per output element and each is half as wide:
+// the reduction that ends the kernel - CTA j PULLS rows 16j .. 16j+15 of the partials of both column halves over
+// distributed shared memory and sums them in rank order (deterministic) - moves 56 KB per CTA instead of 112 KB.
+// Then bias + residual, the layer's final LayerNorm, stores.
+//
+// Warp roles: warps 0-7 = two consumer warpgroups (rows 0-63 / 64-127 of the tile: wgmma, GELU, reduction), warp 8 = TMA
+// producer, warp 9 = exchange with the partner CTA; further warps of a larger CTA only take part in the barriers.
 //
 // Shared memory (192 KB):  R0 [0, 64K)    GEMM 1 stage 0, then the partner's S (same layout as S)
 //                          R1 [64K, 128K) GEMM 1 stage 1, then the W2 ring: 2 slots of 32 KB (k-block of 64: hi 16K | lo 16K)
 //                          S  [128K,192K) S_hi [2][16K] | S_lo [2][16K]
 //                          after GEMM 2: the fp32 partial tile [128][132] at offset 0.
-// TMEM (512 columns): GEMM 1 main [0,128) + small [128,256); GEMM 2 main [256,384) + small [384,512) - disjoint, so GEMM 2
-// starts on the first k-block of S while the epilogue warps still read GEMM 1's accumulators for the second.
 namespace mlp {
 constexpr int FC = 128;                       // hidden columns per CTA
 constexpr int CLUSTER = 8;                    // d_ff / FC
@@ -122,34 +159,12 @@ constexpr int RING = 2 * STAGE1;
 constexpr int S_BYTES = 64 * 1024;            // S_hi [2][16K] | S_lo [2][16K]
 constexpr int W2SLOT = 32 * 1024;             // W2 k-block: hi [128 rows][128 B] | lo
 constexpr int PLD = NH + 4;                   // fp32 partial row stride (floats)
-constexpr int SMEM_BYTES = RING + S_BYTES + 1024 /*alignment slack*/ + 1024 /*barriers, tmem slot*/;
-// barriers (8 B each, above the operand region): full1[2] 0,1 | empty1[2] 2,3 | acc1 4 | w2full[2] 5,6 | s_ready[0] 7 | acc2 8 |
-// s_ready[1] 9 | w2empty[2] 10,11 | peer_free 12 | peer_s hi[2] 13,14 | peer_s lo[2] 15,16 ; tmem slot at 8*17
-constexpr int TMEM_SLOT_OFF = 8 * 17;
+constexpr int SMEM_BYTES = RING + S_BYTES + 1024 /*alignment slack*/ + 1024 /*barriers*/;
+constexpr int CW = 8;                         // consumer warps
+// barriers (8 B each, above the operand region): full1[2] 0,1 | empty1[2] 2,3 | gemm1_done 4 | w2full[2] 5,6 | s_ready[0] 7 |
+// s_ready[1] 9 | w2empty[2] 10,11 | peer_free 12 | peer_s hi[2] 13,14 | peer_s lo[2] 15,16
 }  // namespace mlp
 
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&u)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]), "=r"(u[7]),
-          "=r"(u[8]), "=r"(u[9]), "=r"(u[10]), "=r"(u[11]), "=r"(u[12]), "=r"(u[13]), "=r"(u[14]), "=r"(u[15]),
-          "=r"(u[16]), "=r"(u[17]), "=r"(u[18]), "=r"(u[19]), "=r"(u[20]), "=r"(u[21]), "=r"(u[22]), "=r"(u[23]),
-          "=r"(u[24]), "=r"(u[25]), "=r"(u[26]), "=r"(u[27]), "=r"(u[28]), "=r"(u[29]), "=r"(u[30]), "=r"(u[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// 16 columns of this warp's 32 TMEM lanes, no wait (pair with tmem_ld_wait)
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, uint32_t (&u)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]), "=r"(u[7]),
-          "=r"(u[8]), "=r"(u[9]), "=r"(u[10]), "=r"(u[11]), "=r"(u[12]), "=r"(u[13]), "=r"(u[14]), "=r"(u[15])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
     asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
@@ -164,25 +179,19 @@ struct MlpArgs {
     long long* trace;
 };
 
-// Barriers and the TMEM allocation of the feed-forward block; ends with a CTA barrier.  The barrier
-// words live ABOVE the 192 KB operand region, so a caller may use that region for something else until mlp_run starts.
+// Barriers of the feed-forward block; ends with a CTA barrier.  The barrier words live ABOVE the 192 KB operand region, so
+// a caller may use that region for something else until mlp_run starts.
 // EARLY (stand-alone kernel: the operand region is free from the start): the thread that initialises the barriers also
 // requests the first two k-blocks of operands at once - W1 (step-invariant), then, after the dependency wait, X - instead of
-// leaving that to the producer warp after the TMEM allocation and the CTA barrier.  Most CTAs of a launch only get their SM
-// when the previous kernel's CTAs leave (every kernel of the step fills the SMs' shared memory), so for them nothing overlaps
-// the prologue and these ~700 cycles are on the step's critical path.  mlp_run<EW, true> then skips those requests.
-template <int EW, bool EARLY = false>      // EW = number of epilogue warps of mlp_run<EW>: 8 or 16
-__device__ __forceinline__ uint32_t mlp_setup(uint8_t* smem_raw, const MlpArgs& a, int j = 0, int m0 = 0) {
+// leaving that to the producer warp after the CTA barrier.  mlp_run<true> then skips those requests.
+template <bool EARLY = false>
+__device__ __forceinline__ void mlp_setup(uint8_t* smem_raw, const MlpArgs& a, int j = 0, int m0 = 0) {
     using namespace mlp;
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
     const uint32_t bars = base + RING + S_BYTES;
-    const uint32_t tmem_slot = bars + (uint32_t)TMEM_SLOT_OFF;
-    volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(base_ptr + RING + S_BYTES + TMEM_SLOT_OFF);
-    const int warp = threadIdx.x >> 5;
     if (threadIdx.x == 0) {
         if (EARLY) {
-            // the two "operands landed" barriers of GEMM 1 first, so that the first requests leave before the other 15 barriers exist
+            // the two "operands landed" barriers of GEMM 1 first, so that the first requests leave before the other barriers exist
             mbar_init(bars, 1); mbar_init(bars + 8u, 1);
             asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
             for (int kb = 0; kb < 2; kb++) {
@@ -199,10 +208,13 @@ __device__ __forceinline__ uint32_t mlp_setup(uint8_t* smem_raw, const MlpArgs& 
                 tma_load_2d(dst + 32768, a.map_xl, bars + 8u * kb, kb * BK, m0);
             }
         }
-        for (int s = 0; s < 2; s++) { if (!EARLY) mbar_init(bars + 8u * s, 1); mbar_init(bars + 8u * (2 + s), 1); mbar_init(bars + 8u * (5 + s), 1); }
-        mbar_init(bars + 8u * 4, 1); mbar_init(bars + 8u * 8, 1);
-        mbar_init(bars + 8u * 7, EW * 32); mbar_init(bars + 8u * 9, EW * 32);
-        for (int s = 0; s < 2; s++) { mbar_init(bars + 8u * (10 + s), 1); mbar_init(bars + 8u * (13 + s), 1); mbar_init(bars + 8u * (15 + s), 1); }
+        for (int s = 0; s < 2; s++) {
+            if (!EARLY) mbar_init(bars + 8u * s, 1);
+            mbar_init(bars + 8u * (2 + s), CW); mbar_init(bars + 8u * (5 + s), 1); mbar_init(bars + 8u * (10 + s), CW);
+            mbar_init(bars + 8u * (13 + s), 1); mbar_init(bars + 8u * (15 + s), 1);
+        }
+        mbar_init(bars + 8u * 4, CW);
+        mbar_init(bars + 8u * 7, CW * 32); mbar_init(bars + 8u * 9, CW * 32);
         mbar_init(bars + 8u * 12, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         // the partner's copies of its S k-blocks complete on these four (16 KB each: hi / lo of a k-block)
@@ -216,29 +228,17 @@ __device__ __forceinline__ uint32_t mlp_setup(uint8_t* smem_raw, const MlpArgs& 
         asm volatile("prefetch.tensormap [%0];" ::"l"(a.map_w2) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(a.map_w2l) : "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    return *tmem_slot_ptr;
 }
 
 // The feed-forward block of one 128-row tile on the cluster's 8 CTAs (see the comment above).  j = rank in the cluster =
 // hidden chunk; m0 = first row of the tile; rows >= row_end are neither reduced nor stored (row_end <= M; a tile may hold
-// fewer than 128 live rows when the caller aligns tiles to samples).  Warps 0 / 1 = TMA producer / MMA issuer, warps 2 .. 1 + EW =
-// epilogue; any further warps of the CTA only take part in the cluster barriers.  wait_dep: execute griddepcontrol.wait
-// before the first dependent access (stand-alone launch); a caller that has already waited passes false.
-template <int EW, bool EARLY = false>
-__device__ __forceinline__ void mlp_run(uint8_t* smem_raw, const MlpArgs& a, int j, int m0, int row_end, uint32_t tmem_base, bool wait_dep,
-                                        long long* tr) {
+// fewer than 128 live rows when the caller aligns tiles to samples).  wait_dep: execute griddepcontrol.wait before the first
+// dependent access (stand-alone launch); a caller that has already waited passes false.
+template <bool EARLY = false>
+__device__ __forceinline__ void mlp_run(uint8_t* smem_raw, const MlpArgs& a, int j, int m0, int row_end, bool wait_dep, long long* tr) {
     using namespace mlp;
-    static_assert(EW == 8 || EW == 16, "8 or 16 epilogue warps (2 or 4 per TMEM lane quarter)");
-    constexpr int NEPI = EW * 32;              // epilogue threads
-    constexpr int WPQ = EW / 4;                // warps per TMEM lane quarter
-    constexpr int NPASS = 1024 / NEPI;         // float4 elements of the 16 x 256 reduction slice per thread
+    constexpr int NPASS = 1024 / (CW * 32);    // float4 elements of the 16 x 256 reduction slice per consumer thread
 #define MTRACE(slot) do { if (tr) tr[slot] = clock64(); } while (0)
     const CUtensorMap& map_x = *a.map_x; const CUtensorMap& map_w1 = *a.map_w1; const CUtensorMap& map_xl = *a.map_xl;
     const CUtensorMap& map_w1l = *a.map_w1l; const CUtensorMap& map_w2 = *a.map_w2; const CUtensorMap& map_w2l = *a.map_w2l;
@@ -252,18 +252,18 @@ __device__ __forceinline__ void mlp_run(uint8_t* smem_raw, const MlpArgs& a, int
     const uint32_t bars = base + RING + S_BYTES;
     auto bar_full1 = [&](int s) { return bars + 8u * s; };
     auto bar_empty1 = [&](int s) { return bars + 8u * (2 + s); };
-    const uint32_t bar_acc1 = bars + 8u * 4;
+    const uint32_t bar_g1done = bars + 8u * 4;
     auto bar_w2full = [&](int s) { return bars + 8u * (5 + s); };
     auto bar_sready = [&](int kb) { return bars + 8u * (kb ? 9 : 7); };
-    const uint32_t bar_acc2 = bars + 8u * 8;
     auto bar_w2empty = [&](int s) { return bars + 8u * (10 + s); };
     const uint32_t bar_peer_free = bars + 8u * 12;
     auto bar_peer_s = [&](int kb, int lo) { return bars + 8u * (13 + 2 * lo + kb); };
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int jp = j ^ 1, hcol = j & 1;          // partner CTA (same pair of hidden chunks), this CTA's half of the output columns
+    const bool consumer = warp < CW;
     if (threadIdx.x == 0) MTRACE(1);
 
-    if (warp == 0 && !EARLY) {
+    if (warp == CW && !EARLY) {
         // ===================== TMA producer, first pipeline fill (EARLY: mlp_setup has already requested it) =====================
         if (elect_one()) {
             for (int kb = 0; kb < 2; kb++) {       // weight tiles do not depend on the previous kernel
@@ -285,12 +285,13 @@ __device__ __forceinline__ void mlp_run(uint8_t* smem_raw, const MlpArgs& a, int
         __syncwarp();
     }
     // Every CTA's barriers must exist (mlp_setup) before a partner arrives on them or copies into this CTA's shared memory:
-    // one cluster barrier, arrive here, wait where each role first needs it (the MMA warp only after it has issued GEMM 1), so
-    // that its latency stays off the critical path.
+    // one cluster barrier, arrive here, wait where each role first needs it (the consumers only after GEMM 1), so that its
+    // latency stays off the critical path.
     asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory");      // (mlp_setup's fence.mbarrier_init is the release)
 #define CLUSTER_WAIT() asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory")
 
-    if (warp == 0) {
+    float4 o[NPASS];                     // this thread's elements of the closing reduction (consumers)
+    if (warp == CW) {
         // ===================== TMA producer =====================
         for (int kb = 2; kb < 4; kb++) {
             const int s = kb & 1;
@@ -309,7 +310,7 @@ __device__ __forceinline__ void mlp_run(uint8_t* smem_raw, const MlpArgs& a, int
         // GEMM 1 finished reading the ring: stream this CTA's half of W2's rows (output columns 128 hcol ..) for the pair's
         // 256 hidden columns through the two 32 KB slots of R1, in the order GEMM 2 consumes them: own chunk j (its S is
         // local), then the partner's
-        mbar_wait(bar_acc1, 0);
+        mbar_wait(bar_g1done, 0);
         for (int i = 0; i < 4; i++) {
             const int sl = i & 1;
             if (i >= 2) mbar_wait(bar_w2empty(sl), 0);
@@ -322,215 +323,134 @@ __device__ __forceinline__ void mlp_run(uint8_t* smem_raw, const MlpArgs& a, int
             }
             __syncwarp();
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        const uint32_t idesc1 = (1u << 4) | ((uint32_t)(FC >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-        const uint32_t idesc2 = (1u << 4) | ((uint32_t)(NH >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-        const uint32_t acc1_main = tmem_base, acc1_small = tmem_base + 128u;
-        for (int kb = 0; kb < 4; kb++) {
-            const int s = kb & 1;
-            mbar_wait(bar_full1(s), (kb >> 1) & 1);
-            tc_fence_after();
-            if (kb == 0 && lane == 0) MTRACE(2);
-            const uint32_t st = base + s * STAGE1;
-            const uint64_t dah = make_smem_desc(st), dwh = make_smem_desc(st + 16384);
-            const uint64_t dal = make_smem_desc(st + 32768), dwl = make_smem_desc(st + 49152);
-            if (elect_one()) {
-#pragma unroll
-                for (int kk = 0; kk < BK / UMMA_K; kk++) {
-                    const uint64_t koff = (uint64_t)((kk * UMMA_K * 2) >> 4);
-                    umma_f16(acc1_small, dal + koff, dwh + koff, idesc1, (kb | kk) ? 1u : 0u);
-                    umma_f16(acc1_small, dah + koff, dwl + koff, idesc1, 1u);
-                    umma_f16(acc1_main, dah + koff, dwh + koff, idesc1, (kb | kk) ? 1u : 0u);
-                }
-                umma_commit(bar_empty1(s));
-                if (kb == 3) umma_commit(bar_acc1);
-            }
-            __syncwarp();
-        }
-        if (lane == 0) MTRACE(3);
+    } else if (warp == CW + 1) {
+        // ===================== exchange with the partner CTA =====================
         CLUSTER_WAIT();
         // GEMM 1 complete: R0 may now receive the partner's S (tell it so), and this CTA may copy into the partner's once it says
         // the same
-        mbar_wait(bar_acc1, 0);
-        if (elect_one()) {
-            uint32_t rbar;
-            asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rbar) : "r"(bar_peer_free), "r"(jp));
-            asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(rbar) : "memory");
-        }
+        mbar_wait(bar_g1done, 0);
+        if (elect_one()) mbar_arrive_remote(bar_peer_free, jp);
         __syncwarp();
-        // GEMM 2: [128 x 128] (this CTA's half of the output columns) = S_pair [128 x 256] . W2[half rows, pair's 256 columns]^T.
-        // A = S k-blocks (own: written by the epilogue warps; partner's: copied in), B = W2 k-blocks in the R1 ring.  As soon as
-        // an own k-block is complete it is also sent to the partner.  Order of the additions per accumulator: own chunk, then
-        // the partner's, k ascending - fixed per CTA, independent of M.
-        const uint32_t acc2_main = tmem_base + 256u, acc2_small = tmem_base + 384u;
-        for (int i = 0; i < 4; i++) {
-            const int sl = i & 1, kb = i & 1;
-            uint32_t a_hi;
-            if (i < 2) {
-                mbar_wait(bar_sready(kb), 0);        // all epilogue threads have written (and proxy-fenced) this k-block of S
-                if (i == 0) { mbar_wait(bar_peer_free, 0); if (lane == 0) MTRACE(6); }
-                if (elect_one()) {
-                    uint32_t rdst, rbar_hi, rbar_lo;
-                    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rdst) : "r"(base + kb * 16384), "r"(jp));
-                    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rbar_hi) : "r"(bar_peer_s(kb, 0)), "r"(jp));
-                    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rbar_lo) : "r"(bar_peer_s(kb, 1)), "r"(jp));
-                    asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                                 ::"r"(rdst), "r"(s_base + kb * 16384), "r"(16384u), "r"(rbar_hi) : "memory");
-                    asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                                 ::"r"(rdst + 32768u), "r"(s_base + 32768 + kb * 16384), "r"(16384u), "r"(rbar_lo) : "memory");
-                }
-                __syncwarp();
-                a_hi = s_base + kb * 16384;
-            } else {
-                mbar_wait(bar_peer_s(kb, 0), 0);     // the hi half of the partner's k-block has landed in R0 (the lo half follows)
-                a_hi = base + kb * 16384;
-            }
-            mbar_wait(bar_w2full(sl), (i >> 1) & 1);
-            tc_fence_after();
-            const uint64_t dah = make_smem_desc(a_hi), dal = make_smem_desc(a_hi + 32768);
-            const uint64_t dwh = make_smem_desc(base + STAGE1 + sl * W2SLOT), dwl = make_smem_desc(base + STAGE1 + sl * W2SLOT + 16384);
-            if (i < 2) {
-                if (elect_one()) {
-#pragma unroll
-                    for (int kk = 0; kk < BK / UMMA_K; kk++) {
-                        const uint64_t koff = (uint64_t)((kk * UMMA_K * 2) >> 4);
-                        umma_f16(acc2_small, dal + koff, dwh + koff, idesc2, (i | kk) ? 1u : 0u);
-                        umma_f16(acc2_small, dah + koff, dwl + koff, idesc2, 1u);
-                        umma_f16(acc2_main, dah + koff, dwh + koff, idesc2, (i | kk) ? 1u : 0u);
-                    }
-                    umma_commit(bar_w2empty(sl));
-                }
-                __syncwarp();
-            } else {
-                // partner's k-block: the products that only read its hi half first, the lo x hi products when the lo half is in
-                if (elect_one()) {
-#pragma unroll
-                    for (int kk = 0; kk < BK / UMMA_K; kk++) {
-                        const uint64_t koff = (uint64_t)((kk * UMMA_K * 2) >> 4);
-                        umma_f16(acc2_small, dah + koff, dwl + koff, idesc2, 1u);
-                        umma_f16(acc2_main, dah + koff, dwh + koff, idesc2, 1u);
-                    }
-                }
-                __syncwarp();
-                mbar_wait(bar_peer_s(kb, 1), 0);
-                tc_fence_after();
-                if (elect_one()) {
-#pragma unroll
-                    for (int kk = 0; kk < BK / UMMA_K; kk++) {
-                        const uint64_t koff = (uint64_t)((kk * UMMA_K * 2) >> 4);
-                        umma_f16(acc2_small, dal + koff, dwh + koff, idesc2, 1u);
-                    }
-                    if (i == 3) umma_commit(bar_acc2);
-                }
-                __syncwarp();
-            }
-        }
-        if (lane == 0) MTRACE(7);
-    } else if (warp < 2 + EW) {
-        // ===================== epilogue warps 2 .. 1 + EW =====================
-        const int q = warp & 3, ew = warp - 2;       // TMEM lane quarter, 0..7
-        const int r = q * 32 + lane;                 // tile row owned by this thread
-        CLUSTER_WAIT();
-        if (wait_dep) pdl_wait();
-        mbar_wait(bar_acc1, 0);
-        tc_fence_after();
-        if (threadIdx.x == 64) MTRACE(4);
-        // ---- hidden chunk: bias + GELU -> (hi, lo) fp16 pairs in the swizzled K-major A layout, one k-block of S (64 hidden
-        // columns) at a time on ALL epilogue warps, so that GEMM 2 can start on the first while the second is produced
-        constexpr int CW = 64 / WPQ;                  // columns per warp and k-block: 16 (16 warps) or 32 (8 warps)
-        const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
         for (int kb = 0; kb < 2; kb++) {
-            uint8_t* srow_hi = base_ptr + RING + kb * 16384 + r * 128;
-            uint8_t* srow_lo = srow_hi + 32768;
-#pragma unroll 1
-            for (int cc = (ew >> 2) * CW; cc < (ew >> 2) * CW + CW; cc += 16) {
-                const int c0 = kb * 64 + cc;
-                uint32_t um[16], us[16];
-                tmem_ld16_nowait(trow + (uint32_t)c0, um);
-                tmem_ld16_nowait(trow + (uint32_t)(128 + c0), us);
-                tmem_ld_wait();
-#pragma unroll
-                for (int ch = 0; ch < 2; ch++) {
-                    uint32_t hw[4], lw[4];
-#pragma unroll
-                    for (int e = 0; e < 4; e++) {
-                        const int i0 = ch * 8 + e * 2;
-                        const float2 bb = *reinterpret_cast<const float2*>(b1 + j * FC + c0 + i0);
-                        gelu_split_x2(__uint_as_float(um[i0]), __uint_as_float(um[i0 + 1]), __uint_as_float(us[i0]), __uint_as_float(us[i0 + 1]),
-                                      bb, hw[e], lw[e]);
-                    }
-                    const int pos = (((cc >> 3) + ch) ^ (r & 7)) * 16;
-                    *reinterpret_cast<uint4*>(srow_hi + pos) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                    *reinterpret_cast<uint4*>(srow_lo + pos) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-                }
+            mbar_wait(bar_sready(kb), 0);        // all consumer threads have written (and proxy-fenced) this k-block of S
+            if (kb == 0) mbar_wait(bar_peer_free, 0);
+            if (elect_one()) {
+                uint32_t rdst, rbar_hi, rbar_lo;
+                asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rdst) : "r"(base + kb * 16384), "r"(jp));
+                asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rbar_hi) : "r"(bar_peer_s(kb, 0)), "r"(jp));
+                asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rbar_lo) : "r"(bar_peer_s(kb, 1)), "r"(jp));
+                asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                             ::"r"(rdst), "r"(s_base + kb * 16384), "r"(16384u), "r"(rbar_hi) : "memory");
+                asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                             ::"r"(rdst + 32768u), "r"(s_base + 32768 + kb * 16384), "r"(16384u), "r"(rbar_lo) : "memory");
             }
-            tc_fence_before();
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy S writes -> visible to the tensor core and the bulk copy
-            asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar_sready(kb)) : "memory");
+            __syncwarp();
         }
-        if (threadIdx.x == 64) MTRACE(5);
+    } else if (consumer) {
+        // ===================== consumer warpgroups =====================
+        const int wg = warp >> 2;                                    // rows 64 wg .. of the tile
+        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);      // this thread's accumulator rows: r0 and r0 + 8
+        const int cq = 2 * (lane & 3);                               // ... and columns 8 j + cq, + 1
+        const uint32_t a_off = (uint32_t)wg * 8192u;                 // the warpgroup's 64 rows of a 128-row operand tile
+        {
+            // ---- GEMM 1: hidden chunk [128 x 128] = X [128 x 256] . W1[chunk j]^T
+            float acc[64], accs[64];
+            for (int kb = 0; kb < 4; kb++) {
+                const int s = kb & 1;
+                mbar_wait(bar_full1(s), (kb >> 1) & 1);
+                if (kb == 0 && threadIdx.x == 0) MTRACE(2);
+                const uint32_t st = base + s * STAGE1;
+                wgmma_fence();
+                split_kblock(acc, accs, make_smem_desc(st + a_off), make_smem_desc(st + 32768 + a_off), make_smem_desc(st + 16384),
+                             make_smem_desc(st + 49152), kb == 0, kb == 0);
+                wgmma_commit();
+                wgmma_wait0();
+                __syncwarp();
+                if (lane == 0) { mbar_arrive(bar_empty1(s)); if (kb == 3) mbar_arrive(bar_g1done); }
+            }
+            if (threadIdx.x == 0) MTRACE(3);
+            CLUSTER_WAIT();
+            if (wait_dep) pdl_wait();
+            // ---- bias + GELU -> (hi, lo) fp16 pairs in the swizzled K-major A layout, one k-block of S (64 hidden columns) at a
+            // time, so that GEMM 2 and the copy to the partner can start on the first while the second is produced
+#pragma unroll
+            for (int kb = 0; kb < 2; kb++) {
+#pragma unroll
+                for (int jj = 0; jj < 8; jj++) {
+                    const int jx = kb * 8 + jj;
+                    const float2 bb = *reinterpret_cast<const float2*>(b1 + j * FC + 8 * jx + cq);
+#pragma unroll
+                    for (int hh = 0; hh < 2; hh++) {
+                        const int r = r0 + 8 * hh;
+                        uint32_t hw, lw;
+                        gelu_split_x2(acc[4 * jx + 2 * hh], acc[4 * jx + 2 * hh + 1], accs[4 * jx + 2 * hh], accs[4 * jx + 2 * hh + 1], bb, hw, lw);
+                        uint8_t* p = base_ptr + RING + kb * 16384 + r * 128 + ((jj ^ (r & 7)) * 16) + cq * 2;
+                        *reinterpret_cast<uint32_t*>(p) = hw;
+                        *reinterpret_cast<uint32_t*>(p + 32768) = lw;
+                    }
+                }
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy S writes -> visible to wgmma and the bulk copy
+                mbar_arrive(bar_sready(kb));
+            }
+            if (threadIdx.x == 0) MTRACE(5);
+        }
+        {
+            // ---- GEMM 2: [128 x 128] (this CTA's half of the output columns) = S_pair [128 x 256] . W2[half rows, pair's 256 columns]^T.
+            // A = S k-blocks (own, then the partner's copied into R0), B = W2 k-blocks in the R1 ring.  Order of the additions per
+            // accumulator: own chunk, then the partner's, k ascending - fixed per CTA, independent of M.
+            float acc[64], accs[64];
+            for (int i = 0; i < 4; i++) {
+                const int sl = i & 1, kb = i & 1;
+                uint32_t a_hi;
+                if (i < 2) {
+                    mbar_wait(bar_sready(kb), 0);
+                    a_hi = s_base + kb * 16384;
+                } else {
+                    mbar_wait(bar_peer_s(kb, 0), 0);
+                    mbar_wait(bar_peer_s(kb, 1), 0);
+                    a_hi = base + kb * 16384;
+                }
+                mbar_wait(bar_w2full(sl), (i >> 1) & 1);
+                const uint32_t w2 = base + STAGE1 + sl * W2SLOT;
+                wgmma_fence();
+                split_kblock(acc, accs, make_smem_desc(a_hi + a_off), make_smem_desc(a_hi + 32768 + a_off), make_smem_desc(w2),
+                             make_smem_desc(w2 + 16384), i == 0, i == 0);
+                wgmma_commit();
+                wgmma_wait0();
+                __syncwarp();
+                if (lane == 0) mbar_arrive(bar_w2empty(sl));
+            }
+            if (threadIdx.x == 0) MTRACE(8);
+            // both warpgroups have finished reading the operand buffers: they become the fp32 partial tile
+            asm volatile("bar.sync 1, 256;" ::: "memory");
+#pragma unroll
+            for (int jx = 0; jx < 16; jx++)
+#pragma unroll
+                for (int hh = 0; hh < 2; hh++)
+                    *reinterpret_cast<float2*>(reinterpret_cast<float*>(base_ptr) + (size_t)(r0 + 8 * hh) * PLD + 8 * jx + cq) =
+                        make_float2(fmaf(accs[4 * jx + 2 * hh], 1.0f / 2048.0f, acc[4 * jx + 2 * hh]),
+                                    fmaf(accs[4 * jx + 2 * hh + 1], 1.0f / 2048.0f, acc[4 * jx + 2 * hh + 1]));
+            if (threadIdx.x == 0) MTRACE(9);
+        }
     } else {
         CLUSTER_WAIT();
     }
 #undef CLUSTER_WAIT
     // ===================== cross-CTA reduction over distributed shared memory =====================
-    // Every CTA writes its [128 x 128] fp32 partial product (its half of the output columns, its pair's 256 hidden columns) into
-    // its own (now idle) operand region; after a cluster barrier CTA j PULLS rows 16j .. 16j+15 of all 8 partials - 4 per column
-    // half - with coalesced 16-byte remote loads and sums each half's four in rank order (56 KB per CTA over the SM-to-SM network).
-    const int q = warp & 3, ew = warp - 2;
-    const bool epi = warp >= 2 && warp < 2 + EW;
-    // Closing reduction: this CTA finalises rows 16j .. 16j+15 of the tile.  One WARP per row (rows ew, ew + EW, ..): pass t of a
-    // lane is row ew + EW (t >> 1), column half t & 1, columns 128 (t & 1) + 4 lane .. + 3 - so a warp instruction reads or writes
-    // 512 contiguous bytes and the row's LayerNorm statistics are warp sums (no shared memory, no block barrier).
-    float4 pre_b[NPASS], pre_r[NPASS];       // bias and residual of this thread's output elements (loaded while GEMM 2 runs)
-    if (epi) {
-#pragma unroll
-        for (int t = 0; t < NPASS; t++) {
-            const int rr = ew + EW * (t >> 1), c4 = (t & 1) * 32 + lane;
-            const int row = m0 + j * 16 + rr;
-            pre_b[t] = pre_r[t] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (row < M) {
-                pre_b[t] = *reinterpret_cast<const float4*>(b2 + c4 * 4);
-                // L2 read: in the fused layer kernel these rows were written by other CTAs of this launch
-                pre_r[t] = __ldcg(reinterpret_cast<const float4*>(res + (size_t)row * ldr + c4 * 4));
-            }
-        }
-        mbar_wait(bar_acc2, 0);          // GEMM 2 complete: the operand buffers may be overwritten
-        tc_fence_after();
-        if (threadIdx.x == 64) MTRACE(8);
-        const int r = q * 32 + lane;
-        float* prow = reinterpret_cast<float*>(base_ptr) + (size_t)r * PLD;
-        const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-        for (int c0 = (ew >> 2) * (NH / WPQ); c0 < (ew >> 2) * (NH / WPQ) + NH / WPQ; c0 += 16) {
-            uint32_t um[16], us[16];
-            tmem_ld16_nowait(trow + (uint32_t)(256 + c0), um);
-            tmem_ld16_nowait(trow + (uint32_t)(384 + c0), us);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 16; i += 4)
-                *reinterpret_cast<float4*>(prow + c0 + i) =
-                    make_float4(fmaf(__uint_as_float(us[i]), 1.0f / 2048.0f, __uint_as_float(um[i])),
-                                fmaf(__uint_as_float(us[i + 1]), 1.0f / 2048.0f, __uint_as_float(um[i + 1])),
-                                fmaf(__uint_as_float(us[i + 2]), 1.0f / 2048.0f, __uint_as_float(um[i + 2])),
-                                fmaf(__uint_as_float(us[i + 3]), 1.0f / 2048.0f, __uint_as_float(um[i + 3])));
-        }
-        tc_fence_before();
-        if (threadIdx.x == 64) MTRACE(9);
-    }
+    // Every CTA has written its [128 x 128] fp32 partial product (its half of the output columns, its pair's 256 hidden columns)
+    // into its own (now idle) operand region; after a cluster barrier CTA j PULLS rows 16j .. 16j+15 of all 8 partials - 4 per
+    // column half - with coalesced 16-byte remote loads and sums each half's four in rank order (56 KB per CTA over the SM-to-SM
+    // network).  One WARP per row (rows warp, warp + 8): pass t of a lane is row warp + 8 (t >> 1), column half t & 1, columns
+    // 128 (t & 1) + 4 lane .. + 3 - so a warp instruction reads or writes 512 contiguous bytes and the row's LayerNorm
+    // statistics are warp sums (no shared memory, no block barrier).
     __syncwarp();
     cluster_sync_all();                  // every CTA's partial tile is complete and visible cluster-wide
-    if (threadIdx.x == 64) MTRACE(10);
-    if (epi) {
-        float4 o[NPASS];
-        // one pass = 4 remote loads in flight per thread (measured: 8 in flight is no faster here, 32 thrash the network's queues);
-        // the loop stays rolled for that
-#pragma unroll 1
+    if (threadIdx.x == 0) MTRACE(10);
+    if (consumer) {
+#pragma unroll
         for (int t = 0; t < NPASS; t++) {
-            const int rr = ew + EW * (t >> 1), hh = t & 1;      // column half hh: its partials live in CTAs hh, hh + 2, hh + 4, hh + 6
-            const int row = m0 + j * 16 + rr;
+            const int rr = warp + CW * (t >> 1), hh = t & 1;      // column half hh: its partials live in CTAs hh, hh + 2, hh + 4, hh + 6
+            const int row = m0 + j * 16 + rr, c4 = hh * 32 + lane;
             const uint32_t off = base + (uint32_t)(((j * 16 + rr) * PLD + lane * 4) * 4);   // same offset in every CTA of the cluster
             float4 p[CLUSTER / 2];
 #pragma unroll
@@ -544,19 +464,17 @@ __device__ __forceinline__ void mlp_run(uint8_t* smem_raw, const MlpArgs& a, int
             for (int i = 0; i < CLUSTER / 2; i++) {      // rank order: deterministic
                 acc.x += p[i].x; acc.y += p[i].y; acc.z += p[i].z; acc.w += p[i].w;
             }
-            // select by constant index (t is a runtime loop counter of a deliberately rolled loop)
-#pragma unroll
-            for (int tt = 0; tt < NPASS; tt++)
-                if (t == tt) {
-                    const float4 bb = pre_b[tt], r4 = pre_r[tt];
-                    o[tt] = row < M ? make_float4((acc.x + bb.x) + r4.x, (acc.y + bb.y) + r4.y, (acc.z + bb.z) + r4.z, (acc.w + bb.w) + r4.w)
-                                    : make_float4(0.f, 0.f, 0.f, 0.f);
-                }
+            o[t] = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (row < M) {
+                const float4 bb = *reinterpret_cast<const float4*>(b2 + c4 * 4);
+                // L2 read: in the fused layer kernel these rows were written by other CTAs of this launch
+                const float4 r4 = __ldcg(reinterpret_cast<const float4*>(res + (size_t)row * ldr + c4 * 4));
+                o[t] = make_float4((acc.x + bb.x) + r4.x, (acc.y + bb.y) + r4.y, (acc.z + bb.z) + r4.z, (acc.w + bb.w) + r4.w);
+            }
         }
         // this thread's remote reads are complete (their values were consumed above): arrive on the closing cluster barrier now,
         // wait for it after the LayerNorm and the stores (the operands tie the instruction to the sums of every pass)
-        if (NPASS == 2) asm volatile("barrier.cluster.arrive.release.aligned;" ::"f"(o[0].x), "f"(o[NPASS - 1].x) : "memory");
-        else asm volatile("barrier.cluster.arrive.release.aligned;" ::"f"(o[0].x), "f"(o[1].x), "f"(o[NPASS - 2].x), "f"(o[NPASS - 1].x) : "memory");
+        asm volatile("barrier.cluster.arrive.release.aligned;" ::"f"(o[0].x), "f"(o[1].x), "f"(o[NPASS - 2].x), "f"(o[NPASS - 1].x) : "memory");
         if (ln_w) {
             // the layer's final LayerNorm, fused: a row = the two passes 2g, 2g + 1 of one warp
             const float4 w0 = *reinterpret_cast<const float4*>(ln_w + lane * 4), w1 = *reinterpret_cast<const float4*>(ln_w + 128 + lane * 4);
@@ -574,7 +492,7 @@ __device__ __forceinline__ void mlp_run(uint8_t* smem_raw, const MlpArgs& a, int
         }
 #pragma unroll
         for (int t = 0; t < NPASS; t++) {
-            const int rr = ew + EW * (t >> 1), c4 = (t & 1) * 32 + lane;
+            const int rr = warp + CW * (t >> 1), c4 = (t & 1) * 32 + lane;
             const int row = m0 + j * 16 + rr;
             if (row < M) {
                 *reinterpret_cast<float4*>(Z + (size_t)row * ldz + c4 * 4) = o[t];
@@ -587,23 +505,15 @@ __device__ __forceinline__ void mlp_run(uint8_t* smem_raw, const MlpArgs& a, int
                 }
             }
         }
-        if (threadIdx.x == 64) MTRACE(11);
+        if (threadIdx.x == 0) MTRACE(11);
     } else {
         asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
     }
     __syncwarp();
     asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");      // nobody leaves (and frees / reuses its shared memory) while peers still read it
-    if (threadIdx.x == 64) MTRACE(12);
+    if (threadIdx.x == 0) MTRACE(12);
     __syncthreads();
 #undef MTRACE
 }
-
-__device__ __forceinline__ void mlp_teardown(uint32_t tmem_base) {
-    if ((threadIdx.x >> 5) == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
-    }
-}
-
 
 }  // namespace tc

@@ -13,7 +13,7 @@ def vertex_normals(vertices, faces):
     assert vertices.ndimension() == 3 and faces.ndimension() == 3
     assert vertices.shape[0] == faces.shape[0] and vertices.shape[2] == 3 and faces.shape[2] == 3
     if vertices.device.type != "cuda":
-        raise RuntimeError("interdiff_b200.data.tools needs a CUDA (sm_100a) device: no CPU fallback")
+        raise RuntimeError("interdiff_b200.data.tools needs a CUDA (sm_90a) device: no CPU fallback")
     V = vertices.shape[1]
     f0 = faces[0]
     key = (vertices.device, V, f0.data_ptr(), f0._version, tuple(f0.shape))

@@ -34,7 +34,7 @@ def _shape_arr(shape):
 class Engine:
     def __init__(self, device=None):
         if not torch.cuda.is_available():
-            raise EngineError("interdiff_b200 needs a CUDA (sm_100a) device; there is no CPU fallback")
+            raise EngineError("interdiff_b200 needs a CUDA (sm_90a) device; there is no CPU fallback")
         self.device = torch.device(device if device is not None else "cuda:%d" % torch.cuda.current_device())
         self.lib = _lib.lib()
         self._h = C.c_void_p()

@@ -85,7 +85,7 @@ class SMPL_Layer(Module):
     def engine_for(self, device):
         device = torch.device(device)
         if device.type != "cuda":
-            raise RuntimeError("interdiff_b200.SMPL_Layer runs on a CUDA (sm_100a) device only: no CPU fallback")
+            raise RuntimeError("interdiff_b200.SMPL_Layer runs on a CUDA (sm_90a) device only: no CPU fallback")
         engines = self.__dict__.setdefault("_engines", {})
         if device not in engines:
             engines[device] = Engine(device)

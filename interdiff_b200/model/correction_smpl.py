@@ -35,7 +35,7 @@ class ObjProjector(nn.Module):
         engines = self.__dict__.setdefault("_engines", {})
         device = torch.device(device)
         if device.type != "cuda":
-            raise RuntimeError("interdiff_b200.ObjProjector runs on a CUDA (sm_100a) device only")
+            raise RuntimeError("interdiff_b200.ObjProjector runs on a CUDA (sm_90a) device only")
         if device not in engines:
             engines[device] = Engine(device)
         return self.load_into(engines[device])

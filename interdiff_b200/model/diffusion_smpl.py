@@ -2,7 +2,7 @@
 (:251-284), create_model_and_diffusion (:286-289).
 
 The module tree reproduces the reference's state_dict names exactly (strict checkpoint loading,
-SURVEY.md section 8b) but only holds parameters: forward() runs the sm_100a decoder in
+SURVEY.md section 8b) but only holds parameters: forward() runs the sm_90a decoder in
 libinterdiff_b200.so.  There is no eager/CPU fallback.
 """
 import torch
@@ -39,7 +39,7 @@ class _EngineHost:
     def engine_for(self, device):
         device = torch.device(device)
         if device.type != "cuda":
-            raise RuntimeError("interdiff_b200.MDM runs on a CUDA (sm_100a) device only: no CPU fallback")
+            raise RuntimeError("interdiff_b200.MDM runs on a CUDA (sm_90a) device only: no CPU fallback")
         engines = self.__dict__.setdefault("_engines", {})
         ent = engines.get(device)
         sig = self._signature()

@@ -1,4 +1,4 @@
-"""Mirror of reference tools.py:11-76 point2point_signed on the sm_100a signed-nearest-neighbour
+"""Mirror of reference tools.py:11-76 point2point_signed on the sm_90a signed-nearest-neighbour
 kernel (replaces the chamfer_distance CUDA extension the reference calls at tools.py:45-47)."""
 import torch
 
@@ -10,7 +10,7 @@ _ENGINES = {}
 def _engine(device):
     device = torch.device(device)
     if device.type != "cuda":
-        raise RuntimeError("interdiff_b200.tools needs a CUDA (sm_100a) device: no CPU fallback")
+        raise RuntimeError("interdiff_b200.tools needs a CUDA (sm_90a) device: no CPU fallback")
     if device not in _ENGINES:
         _ENGINES[device] = Engine(device)
     return _ENGINES[device]

@@ -131,10 +131,10 @@ def random_state_dict(shapes, seed=233):
     return synthetic.fill_state_dict(shapes, seed)
 
 
-# ---- real weights exported from the reference checkpoints (git-ignored, travels with gpurun) --
+# ---- real weights exported from the reference checkpoints (a build product, not in git) --
 # plain .npz files of tensors keyed by the reference's state_dict names; INTERDIFF_B200_WEIGHTS overrides the directory
 REF_WEIGHT_DIR = os.environ.get("INTERDIFF_B200_WEIGHTS") or os.path.join(
-    os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "weights_ref")
+    os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref", "weights")
 
 
 def ref_weights_path(name):
@@ -152,7 +152,7 @@ def load_ref_weights(name):
 
 def bench_weights(name, seed=233):
     """{state_dict name: torch tensor} for the benchmarks / probes / smoke run: the exported checkpoint tensors when
-    weights_ref/<name>.npz exists, else seeded random init of the same shapes (the sinusoid tables are always rebuilt).
+    oracle/_ref/weights/<name>.npz exists, else seeded random init of the same shapes (the sinusoid tables are always rebuilt).
     name: diffusion_smpl | diffusion_skeleton | correction_smpl | diffusion_smpl_encoder."""
     import torch
     sd = load_ref_weights(name)

@@ -1,7 +1,7 @@
 """oracle/ -- TEST INFRASTRUCTURE ONLY (not product code).
 
 CPU restatement of the InterDiff sampling hot path (SURVEY.md section 8) used as the
-parity checker for the sm_100a CUDA path in interdiff_b200/.
+parity checker for the sm_90a CUDA path in interdiff_b200/.
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs
 may import this package.  The product package (interdiff_b200/) never imports it and

@@ -10,12 +10,12 @@ past, identical noise tape) through the REFERENCE's own classes (MDM + SpacedDif
   curve "oracle" : oracle.restate (N threads) vs reference (N threads); "oracle_f64": oracle.restate vs reference float64
 
 per step k = 0..99 (timestep i = 99 - k): max|a-b| / max|b| of the sample x_{t-1} after that step.  The output
-(profiles/r2_conditioning_probe.json + .txt) is what tests/test_gpu_parity.py::test_config2_full_loop reads to decide up
+(tests/golden/conditioning_probe.json + .txt) is what tests/test_gpu_configs.py::test_config2_full_loop reads to decide up
 to which step a free-running comparison at 1e-3 is meaningful: the first step where the reference disagrees with
 ITSELF (float32 vs float64, or 1 vs N threads, whichever comes first) by more than 1e-4 (SURVEY 8d "Parity check",
 VERDICT r1 "What's weak" 1).
 
-  python -m oracle.conditioning_probe [--B 64] [--threads 8] [--out profiles/r2_conditioning_probe]
+  python -m oracle.conditioning_probe [--B 64] [--threads 8] [--out tests/golden/conditioning_probe]
 """
 import argparse
 import json
@@ -62,7 +62,7 @@ def main():
     ap.add_argument("--T", type=int, default=30)
     ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--threads", type=int, default=os.cpu_count())
-    ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "r2_conditioning_probe"))
+    ap.add_argument("--out", default=os.path.join(ROOT, "tests", "golden", "conditioning_probe"))
     a = ap.parse_args()
     from interdiff_b200 import synthetic as S
     from oracle import ref_loader as RL

@@ -1,7 +1,7 @@
-"""Export the hot-path tensors of the reference's shipped checkpoints to weights_ref/*.npz
-(git-ignored; travels to the GPU box with the gpurun snapshot like other built artefacts).
+"""Export the hot-path tensors of the reference's shipped checkpoints to oracle/_ref/weights/*.npz
+(a build product, not in git).
 TEST INFRASTRUCTURE: gives the GPU parity tests / bench the trained weights' value distribution.
-Run in the authoring container:  python -m oracle.export_ref_weights
+Run where the reference tree is installed:  python -m oracle.export_ref_weights
 """
 import os
 import sys

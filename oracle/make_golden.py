@@ -1,8 +1,8 @@
-"""Generate tests/golden/*.npz from the reference's OWN classes (imported from /root/reference via
-oracle.shims) -- run in the authoring container:  python -m oracle.make_golden
+"""Generate tests/golden/*.npz from the reference's OWN classes (imported via
+oracle.shims) -- run where the reference tree is installed:  python -m oracle.make_golden
 TEST INFRASTRUCTURE.  Inputs are the seeded synthetic generators of interdiff_b200.synthetic;
 weights are either the seeded random init (portable: regenerated from the seed by the tests) or
-the shipped checkpoints (tests using those need weights_ref, else skip).
+the shipped checkpoints (tests using those need oracle/_ref/weights, else skip).
 """
 import ast
 import os
@@ -168,5 +168,50 @@ def main():
         print(f, os.path.getsize(os.path.join(OUT, f)))
 
 
+LBS_VERTEX_STRIDE = 16      # smplh_lbs.npz keeps every 16th vertex (and every joint) of the reference's SMPL layer output
+
+
+def lbs_inputs():
+    """seeded inputs of the SMPL-H layer comparison (tests/test_oracle_vs_reference.py::test_smplh_lbs)"""
+    g = torch.Generator().manual_seed(1)
+    Fn = 7
+    pose = 0.4 * torch.randn(Fn, 156, generator=g)
+    pose[0, 3:6] = 0  # exercise the |aa + 1e-8| small-angle path
+    return pose, torch.randn(Fn, 10, generator=g), torch.randn(Fn, 3, generator=g)
+
+
+def smooth_inputs():
+    """seeded inputs of the `smooth` comparison (tests/test_oracle_vs_reference.py::test_smooth_and_best_of_samples)"""
+    g = torch.Generator().manual_seed(0)
+    return g, [torch.randn(30, 2, n, generator=g) for n in (6, 159, 12, 9, 3)]
+
+
+def reference_lbs(smplh_np):
+    pose, betas, trans = lbs_inputs()
+    with torch.no_grad():
+        v, j, _, _ = RL.build_smpl_layer(smplh_np)(pose, th_betas=betas, th_trans=trans)
+    return v, j
+
+
+def reference_smooth():
+    path = os.path.join(RL.ref_root(), "interdiff", "eval_smpl_short.py")
+    fn = [n for n in ast.parse(open(path).read()).body if isinstance(n, ast.FunctionDef) and n.name == "smooth"][0]
+    env = {"args": Namespace(future_len=20)}
+    exec(compile(ast.Module(body=[fn], type_ignores=[]), path, "exec"), env)
+    return env["smooth"](*[x.clone() for x in smooth_inputs()[1]])
+
+
+def main_host_side():
+    """smplh_lbs.npz / smooth.npz: outputs of the reference's SMPL layer and of its `smooth`, for the tests that pin the
+    oracle's LBS and the host-side post-processing where the reference tree is not installed"""
+    v, j = reference_lbs(S.make_smplh_model(233))
+    np.savez_compressed(os.path.join(OUT, "smplh_lbs.npz"), verts=v[:, ::LBS_VERTEX_STRIDE].numpy(), jtr=j.numpy())
+    np.savez_compressed(os.path.join(OUT, "smooth.npz"), **{"out%d" % i: o.numpy() for i, o in enumerate(reference_smooth())})
+
+
 if __name__ == "__main__":
-    main()
+    if "--host-side" in sys.argv:
+        main_host_side()
+    else:
+        main()
+        main_host_side()

@@ -1,7 +1,7 @@
-"""Import the reference's own Python classes (from /root/reference, read-only) through the
-shims, for validating oracle.restate and generating golden vectors in THIS container.
-TEST INFRASTRUCTURE (see oracle/__init__.py).  /root/reference does not exist on the GPU
-box: nothing that runs there may call into this module (callers check `available()`).
+"""Import the reference's own Python classes (read-only, from the tree named by INTERDIFF_REF or the default below)
+through the shims, for validating oracle.restate and generating golden vectors.
+TEST INFRASTRUCTURE (see oracle/__init__.py).  The tree is not installed everywhere: nothing on the GPU path may call
+into this module (callers check `available()`).
 """
 import os
 import sys

@@ -4,7 +4,7 @@
 //   mode 1: push with cp.async.bulk.shared::cluster.shared::cta (TMA engine), completion on the receiver's mbarrier
 //   mode 2: push with st.async (remote store + complete_tx on the receiver's mbarrier), 512 threads
 //   mode 3: like 1, the 7 blocks cut into 4 pieces each (28 bulk copies per CTA)
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o interdiff_b200/build/dsmem_bench profiles/dsmem_bench.cu
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o interdiff_b200/build/dsmem_bench profiles/dsmem_bench.cu
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>

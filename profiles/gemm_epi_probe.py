@@ -1,5 +1,5 @@
-"""How much of a small-GEMM launch is epilogue TMEM traffic: time and error of the denoiser's GEMM shapes vs the
-number of round-robin main accumulators (each one is an extra tcgen05.ld pass per output in the epilogue).
+"""Time and error of the denoiser's GEMM shapes vs the number of k-blocks the wgmma GEMM accumulates in the tensor core
+between two fp32 promotions (idb_debug_set_gemm_accumulators).
 usage: python profiles/gemm_epi_probe.py"""
 import ctypes as C
 import os

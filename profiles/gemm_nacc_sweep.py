@@ -1,4 +1,4 @@
-"""Accuracy / time trade-off of the number of round-robin TMEM accumulators in the tcgen05 GEMM."""
+"""Accuracy / time trade-off of the fp32 promotion interval (k-blocks per tensor-core accumulation) of the wgmma GEMM."""
 import os
 import sys
 

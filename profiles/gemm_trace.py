@@ -1,4 +1,4 @@
-"""Per-CTA clock64 timeline + timing of the tcgen05 GEMM pipeline on PRE-SPLIT operands (the path the
+"""Per-CTA clock64 timeline + timing of the wgmma GEMM pipeline on PRE-SPLIT operands (the path the
 denoiser uses) -- debug aid."""
 import ctypes as C
 import itertools

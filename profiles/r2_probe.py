@@ -54,8 +54,8 @@ for wname, sparse in (("dense tail (every bone non-zero)", False), ("<= 4 non-ze
     for backend in ("simt", "tcgen05"):
         eng.set_gemm_backend(backend)
         ms = timed(lambda: eng.lbs(pose, betas, trans, want_jtr=False), n=10, warm=3, flush_l2=True)
-        print("LBS F=%d, weights: %s, %s path: %.3f ms ; algorithmic %.1f MB -> %.0f GB/s (%.1f %% of 6486) ; %.1f GFLOP -> %.1f TFLOP/s" % (
-            F, wname, "fp32 SIMT" if backend == "simt" else "tcgen05 blend + skinning", ms, byt / 1e6, byt / ms / 1e6, byt / ms / 1e6 / 64.861,
+        print("LBS F=%d, weights: %s, %s path: %.3f ms ; algorithmic %.1f MB -> %.0f GB/s (%.1f %% of the 3350 GB/s data-sheet HBM3 rate) ; %.1f GFLOP -> %.1f TFLOP/s" % (
+            F, wname, "fp32 SIMT" if backend == "simt" else "wgmma blend + skinning", ms, byt / 1e6, byt / ms / 1e6, byt / ms / 1e6 / 33.50,
             F * 33.2e-3, F * 33.2e6 / ms / 1e9))
 eng.set_gemm_backend("tcgen05")
 eng.load_body(S.make_smplh_model(233, sparse_weights=True))

@@ -1,6 +1,6 @@
 """Per-kernel SASS instruction summary of libinterdiff_b200.so (cuobjdump -sass): the mnemonics that prove which hardware
-path a kernel uses - UTCHMMA/UTCQMMA (tcgen05.mma), UTMALDG (TMA tensor loads), UBLKCP (bulk copies), LDTM (tcgen05.ld),
-SYNCS (mbarrier), HMMA (legacy mma.sync), FFMA, LDS/STS, LDG/STG, red/atom.   python profiles/sass_summary.py > profiles/r2_sass_summary.txt"""
+path a kernel uses - HGMMA (wgmma), UTMALDG (TMA tensor loads), UBLKCP (bulk copies),
+SYNCS (mbarrier), HMMA (legacy mma.sync), FFMA, LDS/STS, LDG/STG, red/atom.   python profiles/sass_summary.py"""
 import collections
 import os
 import re
@@ -9,7 +9,7 @@ import sys
 
 so = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "interdiff_b200", "libinterdiff_b200.so")
 out = subprocess.run(["cuobjdump", "-sass", so], capture_output=True, text=True).stdout
-KEYS = ["UTCHMMA", "UTCQMMA", "UTMALDG", "UBLKCP", "LDTM", "SYNCS", "UTCBAR", "HMMA", "FFMA", "MUFU", "LDS", "STS", "LDG", "STG", "RED", "ATOM", "SHFL", "BAR", "UCGABAR", "ACQBULK"]
+KEYS = ["HGMMA", "UTMALDG", "UBLKCP", "SYNCS", "HMMA", "FFMA", "MUFU", "LDS", "STS", "LDG", "STG", "RED", "ATOM", "SHFL", "BAR", "UCGABAR", "ACQBULK"]
 cur, counts, total = None, collections.OrderedDict(), {}
 for line in out.splitlines():
     m = re.match(r"\s*Function : (\S+)", line)
@@ -23,7 +23,7 @@ for line in out.splitlines():
         op = m.group(1).split(".")[0]
         total[cur] += 1
         for k in KEYS:
-            if op == k or (k in ("UTCHMMA", "UTCQMMA", "UTMALDG", "UBLKCP", "LDTM", "SYNCS", "HMMA", "UTCBAR", "UCGABAR") and op.startswith(k)):
+            if op == k or (k in ("HGMMA", "UTMALDG", "UBLKCP", "SYNCS", "HMMA", "UCGABAR") and op.startswith(k)):
                 counts[cur][k] += 1
 def demangle(n):
     try:

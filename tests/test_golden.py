@@ -1,7 +1,7 @@
 """Golden vectors produced by the reference's OWN classes (oracle/make_golden.py, committed under
 tests/golden/).  CPU tests pin oracle.restate to them; GPU tests pin the CUDA path (through the
 C ABI) to them directly, with no oracle in between.  '*_ref' fixtures use the shipped checkpoint
-weights exported to weights_ref (skip when absent); '*_random' use the seeded init."""
+weights exported to oracle/_ref/weights (skip when absent); '*_random' use the seeded init."""
 import os
 
 import numpy as np

@@ -41,11 +41,9 @@ def eng():
 
 def _cutoff(default=85):
     """first step k at which the REFERENCE's own classes disagree with themselves on configs[1] by more than 1e-4
-    (float32 vs float64 run, or 1 vs N threads; oracle/conditioning_probe.py -> profiles/r2_conditioning_probe.json:
+    (float32 vs float64 run, or 1 vs N threads; oracle/conditioning_probe.py, a CPU run stored as tests/golden/conditioning_probe.json:
     k = 85; the reference's float32 sample is 0.44 away from its float64 sample at the last step)"""
-    p = os.path.join(ROOT, "profiles", "r2_conditioning_probe.json")
-    if not os.path.exists(p):
-        return default, None
+    p = os.path.join(ROOT, "tests", "golden", "conditioning_probe.json")
     with open(p) as f:
         d = json.load(f)
     return int(d["first_step_self_above_1e4"]), d["reference_f32_vs_f64"]

@@ -17,7 +17,7 @@ def eng():
 
 SHAPES = [(1920, 1024, 256), (1920, 256, 1024), (1920, 768, 256), (1920, 256, 256), (640, 512, 256),
           (100, 72, 36), (129, 200, 100), (1, 8, 4), (300, 1024, 260),
-          (1920, 1536, 256), (2500, 1280, 200)]   # > 148 128-column tiles: the 256-column tile configuration
+          (1920, 1536, 256), (2500, 1280, 200)]   # more 128-column tiles than the H100 has SMs (132): several waves
 
 
 @pytest.mark.parametrize("backend", ["simt", "tcgen05"])

@@ -441,8 +441,9 @@ def test_fused_feed_forward_with_final_norm(eng, M):
 
 def test_launch_structure_switches_bit_identical(eng):
     """The launch-structure options of the step compute every row with the same arithmetic: self- + cross-attention of the
-    standard layers as one launch vs two (idb_set_fused_mlp 11 / 10), 192- vs 256-column tiles of the folded QKV projection
-    (idb_debug_set_gemm_accumulators 901 / 900: same single accumulator and k order per element)."""
+    standard layers as one launch vs two (idb_set_fused_mlp 11 / 10), 128- vs 64-column GEMM tiles
+    (idb_debug_set_gemm_accumulators 901 / 900; the hook keeps its name, other values set the fp32 promotion interval:
+    same operations in the same k order per element whatever the tile width)."""
     sd = mdm_weights("smpl", "auto")
     eng.load_denoiser(sd, "smpl")
     for B2, T2 in ((64, 30), (5, 35), (9, 16)):
