@@ -100,6 +100,13 @@ int idb_pointcloud_embed(idb_handle* h, int B, int P, const float* obj_points, f
  * diffusion/respace.py:64-129 (timestep_map).  betas: the (re-spaced) float64 schedule on the
  * host; timestep_map[n] the model timestep of step index i. */
 int idb_diffusion_init(idb_handle* h, const double* betas, const int64_t* timestep_map, int n);
+/* DDIM instead of DDPM: ddim_sample (gaussian_diffusion.py:738-788) for the START_X model, eq. 12 folded on the host in
+ * float64 onto x_{i-1} = a_i x0 + b_i x_t + sigma_i eps (a_0 = 1, b_0 = 0, sigma_0 = 0 exactly).  Same arguments as
+ * idb_diffusion_init plus eta (>= 0 and finite, else IDB_ERR_ARG; also IDB_ERR_ARG when 1 - alpha_bar_prev - sigma^2 < 0 at
+ * some step).  Replaces the loaded table and drops the captured graphs, like idb_diffusion_init; the table in use is kept
+ * after an argument error.  The per-step entries below (idb_p_sample, idb_p_sample_predict, idb_p_sample_finish) read whichever
+ * table is loaded: with a DDIM table they compute DDIM steps (ddim_sample with clip_denoised=False, or around a hook). */
+int idb_diffusion_init_ddim(idb_handle* h, const double* betas, const int64_t* timestep_map, int n, double eta);
 /* One p_sample at step index i: x_t -> x_{t-1}.  gt/mask (uint8, 1 = keep gt) may be NULL (no
  * inpainting); noise is the eps drawn for this step; x0_out may be NULL. */
 int idb_p_sample(idb_handle* h, int i, const float* x_t, const float* noise, const float* gt,
@@ -119,6 +126,14 @@ int idb_p_sample_finish(idb_handle* h, int i, const float* x0, const float* x_t,
  * reused for any later call of the same (B, T, n, mask present, correction) on fresh tensors. */
 int idb_p_sample_loop(idb_handle* h, const float* tape, const float* gt, const uint8_t* mask,
                       int correction, int use_graph, float* x_out, void* stream);
+/* Whole DDIM loop (ddim_sample_loop, gaussian_diffusion.py:885-999) over the loaded DDIM table (IDB_ERR_STATE otherwise):
+ * x starts as x_T (no initial inpaint blend, :957-972); steps i = n-1 .. 0.  tape: NULL, or n+1 entries laid out as for
+ * idb_p_sample_loop (entry k+1 = eps of the k-th executed step; entry 0 is not read).  NULL is allowed exactly when every
+ * sigma is 0 (eta = 0): then nothing reads noise; NULL with eta > 0 is IDB_ERR_ARG.  clip_denoised != 0 clamps x0 to
+ * [-1, 1] after the inpaint blend / after the hook (process_xstart, :354-360).  correction and use_graph as for
+ * idb_p_sample_loop; the captured graphs are keyed on (B, T, n, mask present, correction, tape present, clip_denoised). */
+int idb_ddim_sample_loop(idb_handle* h, const float* x_T, const float* tape, const float* gt, const uint8_t* mask,
+                         int correction, int clip_denoised, int use_graph, float* x_out, void* stream);
 
 /* ---- SMPL-H linear blend skinning: SMPL_Layer.forward -------------------------------------
  * replaces libsmpl/smplpytorch/pytorch/smpl_layer.py:72-175 (+ rodrigues_layer.py:13-52,

@@ -49,6 +49,8 @@ _SIGS = {
     "idb_p_sample_predict": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, _P]),
     "idb_p_sample_finish": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, _P]),
     "idb_p_sample_loop": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, _P, _P]),
+    "idb_diffusion_init_ddim": (C.c_int, [_P, C.POINTER(C.c_double), C.POINTER(C.c_int64), C.c_int, C.c_double]),
+    "idb_ddim_sample_loop": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
     "idb_body_init": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P]),
     "idb_smplh_lbs": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, _P, _P]),
     "idb_vertex_normals": (C.c_int, [_P, C.c_int, _P, _P, _P]),

@@ -24,10 +24,10 @@ struct DevTensor {
     size_t numel() const { size_t n = 1; for (auto s : shape) n *= (size_t)s; return n; }
 };
 
-struct StepParams {      // one row per diffusion step index i (device table)
+struct StepParams {      // one row per diffusion step index i (device table): x_{i-1} = c1 x0 + c2 x_i + sigma_nz eps
     long long t;         // timestep passed to the model (timestep_map[i])
-    float c1, c2;        // posterior_mean_coef1/2[i]
-    float sigma_nz;      // (i != 0) * exp(0.5 * posterior_log_variance_clipped[i])
+    float c1, c2;        // DDPM: posterior_mean_coef1/2[i]; DDIM: eq. 12 folded onto (x0, x_t), see idb_diffusion_init_ddim
+    float sigma_nz;      // (i != 0) * DDPM exp(0.5 * posterior_log_variance_clipped[i]) / DDIM eta-scaled sigma[i]
     float pad;
 };
 
@@ -92,8 +92,12 @@ struct Denoiser {
     std::vector<float*> bound;              // workspaces to free on rebind
 };
 
+enum { DIFF_DDPM = 0, DIFF_DDIM = 1 };
+
 struct Diffusion {
     int n = 0;
+    int kind = DIFF_DDPM;     // which update the table holds
+    bool noisy = false;       // some step has sigma_nz != 0 (the loop then needs a noise tape)
     std::vector<StepParams> host;
     StepParams* tbl = nullptr;
 };

@@ -929,9 +929,12 @@ k_layer_std_fused(const AttnArgs aa, const XattnArgs xa, const __grid_constant__
 //   HEADS  (mode & 1): lin[(b*T+t)][Clin] -> x0 (B,1,C,T) with the skeleton's keypoint re-derivation and
 //                      the inpainting blend (model/diffusion_smpl.py:245; model/diffusion_skeleton.py:218-248;
 //                      diffusion/gaussian_diffusion.py:307-311)
-//   FINISH (mode & 2): x_{t-1} = c1[i] x0 + c2[i] x_t + sigma[i] eps   (gaussian_diffusion.py:253-275,537-547),
-//                      then - when emit_next - the NEXT step's token pairs and embedding addend, and the
-//                      device step counter moves to i-1 (last block to finish, so nobody still reads it)
+//   FINISH (mode & 2): x_{t-1} = c1[i] x0 + c2[i] x_t + sigma[i] eps   (gaussian_diffusion.py:253-275,537-547; with a
+//                      DDIM table the same expression is eq. 12 of :769-787, folded on the host), then - when
+//                      emit_next - the NEXT step's token pairs and embedding addend, and the device step counter
+//                      moves to i-1 (last block to finish, so nobody still reads it).  noise == null: no eps term and
+//                      no noise load at all (deterministic DDIM); clip: x0 clamped to [-1, 1] where process_xstart
+//                      does it (:354-360) - after the inpainting blend (mode 3) / on the hook's output (mode 2)
 //   TOKENS (mode == 4): x (B,1,C,T) -> token pairs [B*T][Cp] + addend rows, for the first step of a loop and
 //                      for the stand-alone forward
 // addend[b*T+t][:] = (MLP(pe[t_b]) + b_in) + pe[t]  = table row + positional row (model/diffusion_smpl.py:227-232).
@@ -945,11 +948,15 @@ struct StepIO {
     const StepParams* tbl; int* step_cur; int* ticket;
     int tape_mode, n_steps, emit_next;
     int i_host;     // >= 0: the step index, known when the launch is enqueued (else read from step_cur after the dependency wait)
+    int clip;       // clamp x0 to [-1, 1] before the update (clip_denoised)
     // tokens
     const float* x_in; const long long* tstep;
     __half* xtok_b; __half* xtok_s; const float* tab; const float* pe; float* add;
     int pe_rows, T, Clin, C, Cp, variant, c_body, n_points;
 };
+
+// th.clamp(x, -1, 1) (NaN stays NaN)
+__device__ __forceinline__ float clamp_unit(float v) { return v < -1.0f ? -1.0f : (v > 1.0f ? 1.0f : v); }
 
 template <int MODE>
 __global__ void __launch_bounds__(256) k_step_io(const StepIO a) {
@@ -974,7 +981,9 @@ __global__ void __launch_bounds__(256) k_step_io(const StepIO a) {
     auto step_setup = [&]() {
         sp = a.tbl[i_step];
         // tape_mode 0: `noise` is this step's eps; 1: `noise` is the tape (n_steps + 1 entries, [0] = x_T); 2: `noise` is a
-        // device slot holding the tape pointer (captured graphs stay valid when the caller passes a new tape tensor)
+        // device slot holding the tape pointer (captured graphs stay valid when the caller passes a new tape tensor);
+        // null: no noise at all (nz stays null, nothing is loaded)
+        if (!a.noise) return;
         const float* base = a.tape_mode == 2 ? *reinterpret_cast<const float* const*>(a.noise) : a.noise;
         nz = a.tape_mode ? base + (size_t)(a.n_steps - i_step) * ((size_t)gridDim.x * a.C * T) : base;
     };
@@ -985,7 +994,7 @@ __global__ void __launch_bounds__(256) k_step_io(const StepIO a) {
             v_nz[k] = v_gt[k] = 0.f; v_m[k] = 0;
             if (e < n) {
                 const size_t o = ((size_t)b * a.C + c0) * T + e;        // (B,1,C,T): the block's channels are contiguous
-                if (MODE & 2) v_nz[k] = nz[o];
+                if ((MODE & 2) && nz) v_nz[k] = nz[o];
                 if ((MODE & 1) && a.mask) { v_m[k] = a.mask[o]; v_gt[k] = a.gt[o]; }
             }
         }
@@ -1077,11 +1086,16 @@ __global__ void __launch_bounds__(256) k_step_io(const StepIO a) {
                     val = (r0 * zp[0] + r1 * zp[1] + r2 * zp[2]) + tr;
                 }
                 if (v_m[k]) val = v_gt[k];
+                if ((MODE & 2) && a.clip) val = clamp_unit(val);
                 if (a.x0_out) a.x0_out[o] = val;
+            } else if ((MODE & 2) && a.clip) {
+                val = clamp_unit(val);
             }
             if (MODE & 2) {
-                const float mean = sp.c1 * val + sp.c2 * v_xt[k];
-                val = mean + sp.sigma_nz * v_nz[k];
+                // contraction spelled out: the fused tail (mode 3) and the stand-alone finish (mode 2) round identically,
+                // so a loop and its composition from single-step entries give the same bits
+                const float mean = __fmaf_rn(sp.c1, val, __fmul_rn(sp.c2, v_xt[k]));
+                val = __fmaf_rn(sp.sigma_nz, v_nz[k], mean);
                 a.x_next[o] = val;
             }
             if (MODE != 1) tile[cc * LT + t] = val;      // tokens of the step that consumes this tensor
@@ -1755,22 +1769,23 @@ int idb_denoiser_heads(idb_handle* h, const float* gt, const unsigned char* mask
     return launch_step_io<1>(h, a, st);
 }
 
-// posterior sample from a given x0 (after the correction hook, or the stand-alone finish call)
+// posterior sample from a given x0 (after the correction hook, or the stand-alone finish call); noise may be null (no eps
+// term), clip clamps x0 first
 int idb_step_finish(idb_handle* h, const float* x0, const float* xt, const float* noise, int tape_mode, float* x_next, int emit_next,
-                    cudaStream_t st, int i_host) {
+                    cudaStream_t st, int i_host, int clip) {
     StepIO a = step_io_base(h);
     a.i_host = i_host;
-    a.x0_in = x0; a.xt = xt; a.noise = noise; a.tape_mode = tape_mode; a.x_next = x_next; a.emit_next = emit_next;
+    a.x0_in = x0; a.xt = xt; a.noise = noise; a.tape_mode = tape_mode; a.x_next = x_next; a.emit_next = emit_next; a.clip = clip;
     return launch_step_io<2>(h, a, st);
 }
 
 // heads + posterior sample + next step's tokens in one kernel (the tail of a plain sampling step)
 int idb_step_tail(idb_handle* h, const float* gt, const unsigned char* mask, float* x0_out, const float* xt, const float* noise,
-                  int tape_mode, float* x_next, int emit_next, cudaStream_t st, int i_host) {
+                  int tape_mode, float* x_next, int emit_next, cudaStream_t st, int i_host, int clip) {
     StepIO a = step_io_base(h);
     a.i_host = i_host;
     a.gt = gt; a.mask = mask; a.x0_out = x0_out;
-    a.xt = xt; a.noise = noise; a.tape_mode = tape_mode; a.x_next = x_next; a.emit_next = emit_next;
+    a.xt = xt; a.noise = noise; a.tape_mode = tape_mode; a.x_next = x_next; a.emit_next = emit_next; a.clip = clip;
     return launch_step_io<3>(h, a, st);
 }
 

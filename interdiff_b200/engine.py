@@ -47,6 +47,7 @@ class Engine:
         self.variant = None
         self.C = None
         self.n_steps = 0
+        self.diffusion_kind = None     # ("ddpm", None) / ("ddim", eta) of the loaded step table
 
     def close(self):
         if self._h:
@@ -216,6 +217,20 @@ class Engine:
             tm = (C.c_int64 * n)(*[int(v) for v in timestep_map])
         self._chk(self.lib.idb_diffusion_init(self._h, betas.ctypes.data_as(C.POINTER(C.c_double)), tm, n))
         self.n_steps = n
+        self.diffusion_kind = ("ddpm", None)
+
+    def init_diffusion_ddim(self, betas, timestep_map=None, eta=0.0):
+        """DDIM table (ddim_sample, gaussian_diffusion.py:738-788) for the same (re-spaced) schedule: p_sample,
+        p_sample_predict / p_sample_finish then compute DDIM steps and ddim_sample_loop runs the whole loop.  eta = 0 is
+        deterministic (no noise tape needed).  Replaces the loaded table; the next loop re-captures its graphs."""
+        betas = np.ascontiguousarray(betas, dtype=np.float64)
+        n = len(betas)
+        tm = None
+        if timestep_map is not None:
+            tm = (C.c_int64 * n)(*[int(v) for v in timestep_map])
+        self._chk(self.lib.idb_diffusion_init_ddim(self._h, betas.ctypes.data_as(C.POINTER(C.c_double)), tm, n, float(eta)))
+        self.n_steps = n
+        self.diffusion_kind = ("ddim", float(eta))
 
     @staticmethod
     def _mask_u8(mask, device):
@@ -273,6 +288,25 @@ class Engine:
         self._chk(self.lib.idb_p_sample_loop(self._h, self._ptr(tape), self._ptr(gt), self._ptr(m), int(bool(correction)),
                                              int(mode), self._ptr(out), self._stream()))
         self._keep_loop = [tape, gt, m]   # read asynchronously by the enqueued work
+        return out
+
+    def ddim_sample_loop(self, x_T, tape=None, gt=None, mask=None, correction=False, clip_denoised=False, use_graph=True, out=None):
+        """The whole DDIM loop over the table of init_diffusion_ddim, from x_T (B,1,C,T).  tape: None (eta = 0 only) or the
+        (n_steps+1, B,1,C,T) tape of p_sample_loop, whose entry k+1 is the eps of the k-th step (entry 0 is not read).
+        clip_denoised clamps pred_xstart to [-1, 1] after the inpaint blend / the correction hook.  Graphs are cached as for
+        p_sample_loop, per (tape present, clip_denoised) as well."""
+        x_T = self._f32(x_T)
+        if tape is not None:
+            assert tape.is_cuda and tape.dtype == torch.float32 and tape.is_contiguous()
+            assert tape.shape[0] == self.n_steps + 1 and tape.shape[1:] == x_T.shape
+        gt = self._f32(gt) if gt is not None else None
+        m = self._mask_u8(mask, self.device)
+        if out is None:
+            out = torch.empty_like(x_T)
+        self._chk(self.lib.idb_ddim_sample_loop(self._h, self._ptr(x_T), self._ptr(tape), self._ptr(gt), self._ptr(m),
+                                                int(bool(correction)), int(bool(clip_denoised)), int(self._graph_mode(use_graph)),
+                                                self._ptr(out), self._stream()))
+        self._keep_loop = [x_T, tape, gt, m]
         return out
 
     def pointcloud_embed(self, obj_points):
