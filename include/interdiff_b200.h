@@ -33,10 +33,10 @@ int idb_set_gemm_backend(idb_handle* h, int backend); /* 0 = fp32 SIMT (debug/bi
 /* Programmatic dependent launch between the kernels of a sampling step (default 1). Results are identical
    either way; 0 serialises the kernels (for bisecting / profiling). */
 int idb_set_dependent_launch(idb_handle* h, int on);
-/* Feed-forward block of a decoder layer as one cluster kernel (tensor backend, d_model 256, d_ff 1024): 2 (default) = incl.
-   the layer's final LayerNorm in its reduction epilogue, 1 = feed-forward only, 0 = the two separate GEMMs (bisecting);
-   3 = a layer's attention half in the same kernel (option, not faster).  10 / 11: self- and cross-attention of the standard
-   layers as two launches / one launch (default 11; identical results). */
+/* Feed-forward block of a decoder layer: 2 (default) = one cluster kernel incl. the layer's final LayerNorm in its reduction
+   epilogue (tensor backend, d_model 256, d_ff 1024; other configurations run the two GEMMs), 0 = the two separate GEMMs
+   (bisecting).  10 / 11: self- and cross-attention of the standard layers as two launches / one launch (default 11;
+   identical results).  Any other value is IDB_ERR_ARG and changes nothing. */
 int idb_set_fused_mlp(idb_handle* h, int on);
 /* Cluster-pruned nearest-neighbour search when the target is the loaded body mesh (default 1; results are identical
    to the brute-force scan, index ties included); 0 = always brute force. */
@@ -224,8 +224,6 @@ int idb_add_offset(idb_handle* h, int T, int B, int K, long long ld, int col0, f
 
 /* bisecting hook: 0 = the SMPL-H blend GEMM without TMA-multicast row-tile pairs (identical results; default 1) */
 int idb_debug_set_gemm_multicast(idb_handle* h, int on);
-/* profiling hook: 8-CTA clusters of the fused decoder-layer kernel that fit on the device at once (-1 on error) */
-int idb_debug_max_layer_clusters(idb_handle* h);
 
 /* ---- kernel-level hook (tests / bench roofline leg) -----------------------------------------
  * C[M,N] = epi(A[M,K] . W[N,K]^T) with the handle's GEMM backend; epi bit 0 bias, 1 GELU(erf),

@@ -30,7 +30,6 @@ _SIGS = {
     "idb_rollout_next_window": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P]),
     "idb_add_offset": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_longlong, C.c_int, _P, _P, C.c_float, _P]),
     "idb_debug_set_gemm_multicast": (C.c_int, [_P, C.c_int]),
-    "idb_debug_max_layer_clusters": (C.c_int, [_P]),
     "idb_smooth": (C.c_int, [_P, C.c_int, C.c_int, C.c_longlong, _P, _P]),
     "idb_metric_min": (C.c_int, [_P, C.c_longlong, _P, _P, _P]),
     "idb_set_gemm_backend": (C.c_int, [_P, C.c_int]),

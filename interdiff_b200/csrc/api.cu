@@ -83,8 +83,9 @@ extern "C" double idb_debug_last_ms(const idb_handle* h) { return h ? h->last_ms
 extern "C" int idb_set_fused_mlp(idb_handle* h, int on) {
     IDB_ENTER(h);
     if (!h) return IDB_ERR_ARG;
-    if (on == 10 || on == 11) { h->fuse_attn = on - 10; idb_sampler_drop_graphs(h); return IDB_OK; }   /* standard layers: attention halves in one launch */
-    h->fused_mlp = on < 0 ? 0 : (on > 3 ? 3 : on);   /* 0 = two GEMMs, 1 = cluster kernel, 2 = + the layer's final norm, 3 = + the layer's attention half (QaN layers) */
+    if (on == 10 || on == 11) h->fuse_attn = on - 10;     /* standard layers: attention halves in one launch */
+    else if (on == 0 || on == 2) h->fused_mlp = on / 2;   /* 0 = two GEMMs, 2 = cluster kernel incl. the layer's final norm */
+    else return idb_fail(h, IDB_ERR_ARG, "idb_set_fused_mlp: %d is not one of 0, 2, 10, 11", on);
     idb_sampler_drop_graphs(h);
     return IDB_OK;
 }

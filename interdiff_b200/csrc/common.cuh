@@ -118,9 +118,8 @@ struct idb_handle {
     int gemm_multicast = 1;   // long wide GEMMs (SMPL-H blend): row-tile pairs share the W tile by TMA multicast (idb_debug_set_gemm_multicast)
     int nn_pruning = 1;       // cluster-pruned nearest-neighbour search for body-mesh targets (identical results)
     int fuse_attn = 1;        // standard decoder layers: self-attention + cross-attention in one launch (idb_set_fused_mlp(h, 10 / 11) = off / on)
-    int fused_mlp = 2;        // feed-forward block as ONE cluster kernel (tensor backend, d_model 256, d_ff 1024); 2 = incl. the layer's final norm;
-                              // 3 = a layer's attention half runs in the same kernel on sample-aligned tiles (one launch per layer) -
-                              // an option: programmatic dependent launch already hides most of the boundary
+    int fused_mlp = 1;        // feed-forward block + the layer's final norm as ONE cluster kernel (tensor backend, d_model 256, d_ff 1024);
+                              // 0 = two GEMMs with the norm left to the next kernel (idb_set_fused_mlp(h, 2 / 0) = on / off)
     void* metrics_ws = nullptr; size_t metrics_bytes = 0;        // workspace of idb_metrics (posed object points, normals, signed distances)
     void* scratch = nullptr; size_t scratch_bytes = 0;   // on-the-fly operand splits of idb_gemm
     Denoiser den;

@@ -7,7 +7,6 @@
 // is what the 3-tap QaN filter and the per-sample attention want), features contiguous.
 // All arithmetic fp32 (see gemm.cu header for why).
 #include "common.cuh"
-#include "tc_mlp.cuh"
 
 #include <cstdarg>
 
@@ -569,7 +568,7 @@ struct XattnArgs {
     const float* x1; const uint8_t* mpack; const float *bo, *lnw, *lnb;      // mpack: k_pack_memory's per-sample blocks
     float* out; __half *out_b, *out_s; int T, B, Tk, H;
 };
-// own_rows: the x1 rows were written by THIS CTA with plain stores just before (fused standard layer): read them back with
+// own_rows: the x1 rows were written by THIS CTA with plain stores just before (k_attn_xattn_ln): read them back with
 // plain L2 loads instead of bulk copies (which would need a proxy fence)
 __device__ __forceinline__ void xattn_body(const XattnArgs& xa, float* sm, const int b, const int r0, const bool own_rows) {
     const float* __restrict__ x1 = xa.x1;
@@ -657,7 +656,7 @@ struct QanArgs {
     const uint8_t* mpack; const float *bo2, *ln2w, *ln2b; float* out; __half *out_b, *out_s; int T, N, B, Tk, H;   // mpack: k_pack_memory's blocks
 };
 // the slab (sample b, rows r0 .. r0 + 15) of the kernel below as a device function on caller-provided shared memory `sm`
-// (16-byte aligned, qan_smem() bytes): also phase A of the fused decoder-layer kernel
+// (16-byte aligned, qan_smem() bytes)
 // PRELN = false: instantiated without the pending-LayerNorm code (the fused feed-forward kernel applies the previous layer's
 // norm3 itself, so the hot path never has one pending; a skipped block of ~150 instructions still costs its instruction fetches)
 template <bool XATTN, bool PRELN = true>
@@ -837,89 +836,6 @@ k_qan_xattn_ln(const QanArgs qa) {
     if (threadIdx.x == 0) chain_mark(3, 0);
     qan_xattn_body<XATTN, PRELN>(qa, sm, blockIdx.x, blockIdx.y * SLAB);
     if (c_chain) { __syncthreads(); if (threadIdx.x == 0) chain_mark(3, 2); }
-}
-
-// ---------------------------------------------------------------------------------------------
-// One QaN decoder layer in ONE launch: QaN block + LN1 + cross-attention + LN2 (phase A, the kernel above as a device
-// function) and the feed-forward block + the layer's final LayerNorm (phase B, tc::mlp_run).  A cluster of 8 CTAs owns G whole
-// samples (G = 8 / ceil(T / 16): 4 samples = 120 rows for T = 30): in phase A CTA c takes slab c % nslabs of the cluster's
-// sample c / nslabs; the LN2 rows (fp32 for the residual, fp16 pairs for the tensor core) go to global memory (L2); after a
-// cluster barrier the same 8 CTAs run the feed-forward block on the cluster's rows as one 128-row tile (rows past G T belong to
-// the next cluster: computed, never reduced or stored).  Tiles aligned to samples mean NO dependency between clusters, so the
-// kernel boundary between the two halves of a layer disappears.  The attention phase uses the operand region of the
-// feed-forward block as its shared memory; the feed-forward barriers sit above it and are set up at entry.
-__global__ void __cluster_dims__(tc::mlp::CLUSTER, 1, 1) __launch_bounds__(ANT, 1)
-k_layer_qan_fused(const QanArgs qa, const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w1,
-                  const __grid_constant__ CUtensorMap map_xl, const __grid_constant__ CUtensorMap map_w1l,
-                  const __grid_constant__ CUtensorMap map_w2, const __grid_constant__ CUtensorMap map_w2l,
-                  const float* __restrict__ b1, const float* __restrict__ b2, const float* __restrict__ res, float* __restrict__ Z,
-                  const float* __restrict__ ln_w, const float* __restrict__ ln_b, __half* __restrict__ Zh, __half* __restrict__ Zl,
-                  int M, int G, int nslabs) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    pdl_trigger();
-    const int c = blockIdx.x, cl = blockIdx.y, tid = threadIdx.x;
-    tc::MlpArgs a{&map_x, &map_w1, &map_xl, &map_w1l, &map_w2, &map_w2l, b1, b2, res, D, Z, D, ln_w, ln_b, Zh, Zl, nullptr};
-    tc::mlp_setup(smem_raw, a);
-    // ---- phase A
-    const int sl = c / nslabs, b = cl * G + sl;
-    const bool attend = sl < G && b < qa.B;
-    if (attend) qan_xattn_body<true>(qa, reinterpret_cast<float*>(smem_raw), b, (c % nslabs) * SLAB);
-    else pdl_wait();
-    // this CTA's rows (plain stores) must be visible to the TMA reads and plain loads of the whole cluster
-    __threadfence();
-    asm volatile("fence.proxy.async;" ::: "memory");
-    __syncthreads();
-    if (tid == 0 && attend) {   // the attention phase's two mbarriers sit in memory the operand ring is about to overwrite
-        asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(smem_addr(smem_raw)) : "memory");
-        asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(smem_addr(smem_raw) + 8u) : "memory");
-    }
-    tc::cluster_sync_all();
-    asm volatile("fence.proxy.async;" ::: "memory");
-    // ---- phase B
-    const int m0 = cl * G * qa.T;
-    tc::mlp_run(smem_raw, a, c, m0, min(M, m0 + G * qa.T), false, nullptr);
-}
-
-// The same for a standard decoder layer (layers 0 and 7): self-attention + LN1 (phase A1, on the folded-QKV projection a
-// GEMM launch produced), cross-attention + LN2 (phase A2, on the rows phase A1 just wrote), feed-forward + LN3 (phase B).
-__global__ void __cluster_dims__(tc::mlp::CLUSTER, 1, 1) __launch_bounds__(ANT, 1)
-k_layer_std_fused(const AttnArgs aa, const XattnArgs xa, const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w1,
-                  const __grid_constant__ CUtensorMap map_xl, const __grid_constant__ CUtensorMap map_w1l,
-                  const __grid_constant__ CUtensorMap map_w2, const __grid_constant__ CUtensorMap map_w2l,
-                  const float* __restrict__ b1, const float* __restrict__ b2, const float* __restrict__ res, float* __restrict__ Z,
-                  const float* __restrict__ ln_w, const float* __restrict__ ln_b, __half* __restrict__ Zh, __half* __restrict__ Zl,
-                  int M, int G, int nslabs) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    pdl_trigger();
-    const int c = blockIdx.x, cl = blockIdx.y, tid = threadIdx.x;
-    tc::MlpArgs a{&map_x, &map_w1, &map_xl, &map_w1l, &map_w2, &map_w2l, b1, b2, res, D, Z, D, ln_w, ln_b, Zh, Zl, nullptr};
-    tc::mlp_setup(smem_raw, a);
-    const int sl = c / nslabs, b = cl * G + sl, r0 = (c % nslabs) * SLAB;
-    const bool attend = sl < G && b < xa.B;
-    float* sm = reinterpret_cast<float*>(smem_raw);
-    if (attend) {
-        attn_body(aa, sm, b, r0);
-        __syncthreads();                 // every warp's LN1 rows are in global memory (same CTA reads them back below)
-        if (tid == 0) {
-            asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(smem_addr(smem_raw)) : "memory");
-            asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(smem_addr(smem_raw) + 8u) : "memory");
-        }
-        __syncthreads();
-        xattn_body(xa, sm, b, r0, true);
-    } else {
-        pdl_wait();
-    }
-    __threadfence();
-    asm volatile("fence.proxy.async;" ::: "memory");
-    __syncthreads();
-    if (tid == 0 && attend) {
-        asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(smem_addr(smem_raw)) : "memory");
-        asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(smem_addr(smem_raw) + 8u) : "memory");
-    }
-    tc::cluster_sync_all();
-    asm volatile("fence.proxy.async;" ::: "memory");
-    const int m0 = cl * G * xa.T;
-    tc::mlp_run(smem_raw, a, c, m0, min(M, m0 + G * xa.T), false, nullptr);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1147,21 +1063,6 @@ __global__ void __launch_bounds__(256) k_step_io(const StepIO a) {
 
 CHAIN_SETTER(idb_chain_set_denoiser)
 
-/* test / profiling hook: how many 8-CTA clusters of the fused decoder-layer kernel the device can hold at once */
-extern "C" int idb_debug_max_layer_clusters(idb_handle* h) {
-    IDB_ENTER(h);
-    if (!h) return -1;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(tc::mlp::CLUSTER, 64); cfg.blockDim = dim3(ANT); cfg.dynamicSmemBytes = tc::mlp::SMEM_BYTES;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = tc::mlp::CLUSTER; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    int n = -1;
-    if (cudaOccupancyMaxActiveClusters(&n, k_layer_qan_fused, &cfg) != cudaSuccess) { cudaGetLastError(); return -1; }
-    return n;
-}
-
 extern "C" int idb_debug_attn_trace(long long* out16) {
     if (!out16) return IDB_ERR_ARG;
     return cudaMemcpyFromSymbol(out16, g_attn_trace, sizeof(long long) * 16) == cudaSuccess ? IDB_OK : IDB_ERR_CUDA;
@@ -1172,9 +1073,6 @@ extern "C" int idb_debug_attn_trace(long long* out16) {
 // ------------------------------------------------------------------------------------------
 
 int idb_pointnet_commit(idb_handle* h);
-// six tensor maps of the feed-forward block (x hi/lo rows [M][256], w1 hi/lo [1024][256], w2 hi/lo [256][1024]); gemm_wgmma.cu
-int idb_mlp_make_maps(idb_handle* h, const __half* x_hi, const __half* x_lo, const __half* w1_hi, const __half* w1_lo, const __half* w2_hi,
-                      const __half* w2_lo, int M, CUtensorMap* out6);
 void idb_pointnet_release(idb_handle* h);
 
 int idb_fail(idb_handle* h, int code, const char* fmt, ...) {
@@ -1627,17 +1525,6 @@ static int denoiser_layers(idb_handle* h, cudaStream_t st) {
             qa.qpack = L.qt_pack; qa.wk = L.wk; qa.lnw = L.ln1w; qa.lnb = L.ln1b; qa.mpack = reinterpret_cast<const uint8_t*>(L.mem_pack);
             qa.bo2 = L.b_oc; qa.ln2w = L.ln2w; qa.ln2b = L.ln2b; qa.out = d.h2; qa.out_b = d.h2_b; qa.out_s = d.h2_s;
             qa.T = T; qa.N = N; qa.B = B; qa.Tk = Tm; qa.H = H;
-            if (fused && h->fused_mlp >= 3 && !pending && qan_smem(Tm, H) <= (size_t)(tc::mlp::RING + tc::mlp::S_BYTES)) {
-                // the whole layer in one cluster kernel (attention phase + feed-forward phase on sample-aligned row tiles)
-                const int nslabs = (T + SLAB - 1) / SLAB, G = tc::mlp::CLUSTER / nslabs;
-                CUtensorMap mp[6];
-                if ((rc = idb_mlp_make_maps(h, d.h2_b, d.h2_s, L.w1_b, L.w1_s, L.w2_b, L.w2_s, M, mp))) return rc;
-                idb_launch(pdl, k_layer_qan_fused, dim3(tc::mlp::CLUSTER, (B + G - 1) / G), ANT, (size_t)tc::mlp::SMEM_BYTES, st, qa,
-                           mp[0], mp[1], mp[2], mp[3], mp[4], mp[5], (const float*)L.b1, (const float*)L.b2, (const float*)d.h2, d.h,
-                           (const float*)L.ln3w, (const float*)L.ln3b, d.h_b, d.h_s, M, G, nslabs);
-                LAUNCH_CHECK(h);
-                continue;
-            }
             // QaN block + LN1 + cross-attention + LN2 in one kernel: (z | h) -> (d.h2, pairs)
             if (pending) idb_launch(pdl, k_qan_xattn_ln<true, true>, slab_grid, ANT, qan_smem(Tm, H), st, qa);
             else idb_launch(pdl, k_qan_xattn_ln<true, false>, slab_grid, ANT, qan_smem(Tm, H), st, qa);
@@ -1656,18 +1543,6 @@ static int denoiser_layers(idb_handle* h, cudaStream_t st) {
             XattnArgs xa = {};
             xa.x1 = d.qc; xa.mpack = reinterpret_cast<const uint8_t*>(L.mem_pack); xa.bo = L.b_oc;
             xa.lnw = L.ln2w; xa.lnb = L.ln2b; xa.out = d.h2; xa.out_b = d.h2_b; xa.out_s = d.h2_s; xa.T = T; xa.B = B; xa.Tk = Tm; xa.H = H;
-            if (fused && h->fused_mlp >= 3 && attn_smem(T, H) <= (size_t)(tc::mlp::RING + tc::mlp::S_BYTES) &&
-                xattn_smem(Tm, H) <= (size_t)(tc::mlp::RING + tc::mlp::S_BYTES)) {
-                // self-attention + cross-attention + feed-forward of the layer in one cluster kernel
-                const int nslabs = (T + SLAB - 1) / SLAB, G = tc::mlp::CLUSTER / nslabs;
-                CUtensorMap mp[6];
-                if ((rc = idb_mlp_make_maps(h, d.h2_b, d.h2_s, L.w1_b, L.w1_s, L.w2_b, L.w2_s, M, mp))) return rc;
-                idb_launch(pdl, k_layer_std_fused, dim3(tc::mlp::CLUSTER, (B + G - 1) / G), ANT, (size_t)tc::mlp::SMEM_BYTES, st, aa, xa,
-                           mp[0], mp[1], mp[2], mp[3], mp[4], mp[5], (const float*)L.b1, (const float*)L.b2, (const float*)d.h2, d.h,
-                           (const float*)L.ln3w, (const float*)L.ln3b, d.h_b, d.h_s, M, G, nslabs);
-                LAUNCH_CHECK(h);
-                continue;
-            }
             if (h->fuse_attn) {
                 // self-attention + LN1 and cross-attention + LN2 in one launch: h -> (d.qc) -> (d.h2, pairs)
                 const size_t smem = attn_smem(T, H) > xattn_smem(Tm, H) ? attn_smem(T, H) : xattn_smem(Tm, H);
@@ -1681,26 +1556,22 @@ static int denoiser_layers(idb_handle* h, cudaStream_t st) {
                 LAUNCH_CHECK(h);
             }
         }
-        // ---- feed forward on x2 = d.h2: ff = gelu(x2 W1^T + b1) kept as pairs only; z = ff W2^T + b2 + x2  (pre-norm3)
+        // ---- feed forward on x2 = d.h2
         if (fused) {
             // both GEMMs, GELU, the residual AND the layer's norm3 in one cluster kernel: the hidden activations never
             // leave the SM and the next layer starts from normalised rows (fp32 + fp16 pairs)
-            if (h->fused_mlp >= 2) {
-                if ((rc = idb_mlp_wgmma(h, d.h2_b, d.h2_s, L.w1_b, L.w1_s, L.b1, L.w2_b, L.w2_s, L.b2, d.h2, D, d.h, D, M, h->pdl, st,
-                                          L.ln3w, L.ln3b, d.h_b, d.h_s)))
-                    return rc;
-                continue;
-            }
-            if ((rc = idb_mlp_wgmma(h, d.h2_b, d.h2_s, L.w1_b, L.w1_s, L.b1, L.w2_b, L.w2_s, L.b2, d.h2, D, d.z, D, M, h->pdl, st)))
+            if ((rc = idb_mlp_wgmma(h, d.h2_b, d.h2_s, L.w1_b, L.w1_s, L.b1, L.w2_b, L.w2_s, L.b2, d.h2, D, d.h, D, M, h->pdl, st,
+                                      L.ln3w, L.ln3b, d.h_b, d.h_s)))
                 return rc;
-        } else {
-            // ff1 also clears d.z (dead here) so that ff2 can run split-K = 2 and fill 120 SMs instead of 60
-            if ((rc = linear(h, d.h2_b, d.h2_s, D, L.w1_b, L.w1_s, D, L.b1, nullptr, nullptr, d.ff_b, d.ff_s, F, M, F, D, EPI_BIAS | EPI_GELU, st,
-                             1, d.z)))
-                return rc;
-            if ((rc = linear(h, d.ff_b, d.ff_s, F, L.w2_b, L.w2_s, F, L.b2, d.h2, d.z, nullptr, nullptr, D, M, D, F, EPI_BIAS | EPI_RES, st, 2)))
-                return rc;
+            continue;
         }
+        // ff = gelu(x2 W1^T + b1) kept as pairs only; z = ff W2^T + b2 + x2  (pre-norm3).  ff1 also clears d.z (dead here) so
+        // that ff2 can run split-K = 2 and fill 120 SMs instead of 60
+        if ((rc = linear(h, d.h2_b, d.h2_s, D, L.w1_b, L.w1_s, D, L.b1, nullptr, nullptr, d.ff_b, d.ff_s, F, M, F, D, EPI_BIAS | EPI_GELU, st,
+                         1, d.z)))
+            return rc;
+        if ((rc = linear(h, d.ff_b, d.ff_s, F, L.w2_b, L.w2_s, F, L.b2, d.h2, d.z, nullptr, nullptr, D, M, D, F, EPI_BIAS | EPI_RES, st, 2)))
+            return rc;
         // QaN layers return tgt + (x - tgt) (model/sublayers.py:338-339); that differs from x by
         // <= 1 ulp of max(|x|,|tgt|) and is not reproduced (DESIGN.md "Deviations").
         pending = &L;
@@ -1802,8 +1673,6 @@ int idb_denoiser_prepare_kernels(idb_handle* h) {
     // opt in to > 48 KB dynamic shared memory once (T <= 36, Tm <= 16 supported: the self-attention slab kernel keeps all folded values of a sample, 4*T*256 floats, in shared memory)
     CUDA_TRY(h, cudaFuncSetAttribute(k_qan_xattn_ln<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)qan_smem(16, 4)));
     CUDA_TRY(h, cudaFuncSetAttribute(k_qan_xattn_ln<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)qan_smem(16, 4)));
-    CUDA_TRY(h, cudaFuncSetAttribute(k_layer_qan_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::mlp::SMEM_BYTES));
-    CUDA_TRY(h, cudaFuncSetAttribute(k_layer_std_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::mlp::SMEM_BYTES));
     CUDA_TRY(h, cudaFuncSetAttribute(k_qan_xattn_ln<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)qan_enc_smem()));
     CUDA_TRY(h, cudaFuncSetAttribute(k_xattn_ln, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)xattn_smem(16, 4)));
     CUDA_TRY(h, cudaFuncSetAttribute(k_attn_ln, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_smem(36, 4)));
@@ -1918,20 +1787,15 @@ extern "C" int idb_encode_condition(idb_handle* h, int B, int Tp, const float* p
             LAUNCH_CHECK(h);
         }
         if (fused) {
-            if (h->fused_mlp >= 2) {
-                if ((rc = idb_mlp_wgmma(h, d.e_h2_b, d.e_h2_s, L.w1_b, L.w1_s, L.b1, L.w2_b, L.w2_s, L.b2, d.e_h2, D, d.e_h, D, M, h->pdl,
-                                          st, L.ln3w, L.ln3b, d.e_h_b, d.e_h_s)))
-                    return rc;
-                continue;
-            }
-            if ((rc = idb_mlp_wgmma(h, d.e_h2_b, d.e_h2_s, L.w1_b, L.w1_s, L.b1, L.w2_b, L.w2_s, L.b2, d.e_h2, D, d.e_z, D, M, h->pdl, st)))
+            if ((rc = idb_mlp_wgmma(h, d.e_h2_b, d.e_h2_s, L.w1_b, L.w1_s, L.b1, L.w2_b, L.w2_s, L.b2, d.e_h2, D, d.e_h, D, M, h->pdl,
+                                      st, L.ln3w, L.ln3b, d.e_h_b, d.e_h_s)))
                 return rc;
-        } else {
-            if ((rc = linear(h, d.e_h2_b, d.e_h2_s, D, L.w1_b, L.w1_s, D, L.b1, nullptr, nullptr, d.e_ff_b, d.e_ff_s, F, M, F, D,
-                             EPI_BIAS | EPI_GELU, st))) return rc;
-            if ((rc = linear(h, d.e_ff_b, d.e_ff_s, F, L.w2_b, L.w2_s, F, L.b2, d.e_h2, d.e_z, nullptr, nullptr, D, M, D, F, EPI_BIAS | EPI_RES, st)))
-                return rc;
+            continue;
         }
+        if ((rc = linear(h, d.e_h2_b, d.e_h2_s, D, L.w1_b, L.w1_s, D, L.b1, nullptr, nullptr, d.e_ff_b, d.e_ff_s, F, M, F, D,
+                         EPI_BIAS | EPI_GELU, st))) return rc;
+        if ((rc = linear(h, d.e_ff_b, d.e_ff_s, F, L.w2_b, L.w2_s, F, L.b2, d.e_h2, d.e_z, nullptr, nullptr, D, M, D, F, EPI_BIAS | EPI_RES, st)))
+            return rc;
         pending = &L;
     }
     // last norm (or, when the fused feed-forward kernel already applied it, a plain copy) into the (Tp,B,D) layout

@@ -231,9 +231,8 @@ mlp_fused_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
     if (threadIdx.x == 0) chain_mark(2, 0);
     pdl_trigger();
     extern __shared__ uint8_t smem_raw[];
-    MlpArgs a{&map_x, &map_w1, &map_xl, &map_w1l, &map_w2, &map_w2l, b1, b2, res, ldr, Z, ldz, ln_w, ln_b, Zh, Zl, trace};
-    mlp_setup<true>(smem_raw, a, blockIdx.x, blockIdx.y * BM);
-    mlp_run<true>(smem_raw, a, blockIdx.x, blockIdx.y * BM, M, true, tr);
+    MlpArgs a{&map_x, &map_w1, &map_xl, &map_w1l, &map_w2, &map_w2l, b1, b2, res, ldr, Z, ldz, ln_w, ln_b, Zh, Zl};
+    mlp_tile(smem_raw, a, blockIdx.x, blockIdx.y * BM, M, tr);
     if (threadIdx.x == 0) chain_mark(2, 2);
 }
 
@@ -349,20 +348,6 @@ int idb_gemm_wgmma(idb_handle* h, const GemmArgs& g, cudaStream_t st) {
 // final LayerNorm (ln_w / ln_b) and an additional fp16 (hi, lo) copy of the output (Z_hi / Z_lo) for the next GEMM.
 bool idb_mlp_wgmma_supported(int d_model, int d_ff) { return d_model == mlp::DM && d_ff == mlp::FC * mlp::CLUSTER; }
 
-// order: x_hi, w1_hi, x_lo, w1_lo, w2_hi, w2_lo (the kernels' parameter order)
-int idb_mlp_make_maps(idb_handle* h, const __half* x_hi, const __half* x_lo, const __half* w1_hi, const __half* w1_lo, const __half* w2_hi,
-                      const __half* w2_lo, int M, CUtensorMap* out6) {
-    const int F = mlp::FC * mlp::CLUSTER;
-    int rc;
-    if ((rc = make_map(h, &out6[0], x_hi, M, mlp::DM, mlp::DM, BM))) return rc;
-    if ((rc = make_map(h, &out6[1], w1_hi, F, mlp::DM, mlp::DM, mlp::FC))) return rc;
-    if ((rc = make_map(h, &out6[2], x_lo, M, mlp::DM, mlp::DM, BM))) return rc;
-    if ((rc = make_map(h, &out6[3], w1_lo, F, mlp::DM, mlp::DM, mlp::FC))) return rc;
-    // W2: boxes of 128 rows (one CTA's half of the output columns) x 64 hidden columns
-    if ((rc = make_map(h, &out6[4], w2_hi, mlp::DM, F, F, mlp::NH))) return rc;
-    return make_map(h, &out6[5], w2_lo, mlp::DM, F, F, mlp::NH);
-}
-
 int idb_mlp_wgmma(idb_handle* h, const __half* x_hi, const __half* x_lo, const __half* w1_hi, const __half* w1_lo, const float* b1,
                     const __half* w2_hi, const __half* w2_lo, const float* b2, const float* res, int ldr, float* Z, int ldz, int M,
                     int pdl, cudaStream_t st, const float* ln_w, const float* ln_b, __half* Z_hi, __half* Z_lo) {
@@ -379,6 +364,7 @@ int idb_mlp_wgmma(idb_handle* h, const __half* x_hi, const __half* x_lo, const _
     if ((rc = make_map(h, &mxl, x_lo, M, mlp::DM, mlp::DM, BM))) return rc;
     if ((rc = make_map(h, &mw1, w1_hi, F, mlp::DM, mlp::DM, mlp::FC))) return rc;
     if ((rc = make_map(h, &mw1l, w1_lo, F, mlp::DM, mlp::DM, mlp::FC))) return rc;
+    // W2: boxes of 128 rows (one CTA's half of the output columns) x 64 hidden columns
     if ((rc = make_map(h, &mw2, w2_hi, mlp::DM, F, F, mlp::NH))) return rc;
     if ((rc = make_map(h, &mw2l, w2_lo, mlp::DM, F, F, mlp::NH))) return rc;
     dim3 grid(mlp::CLUSTER, (M + BM - 1) / BM);

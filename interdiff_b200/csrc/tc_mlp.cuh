@@ -1,5 +1,5 @@
-// wgmma / TMA / mbarrier PTX wrappers and the fused feed-forward block as a device function, shared by
-// gemm_wgmma.cu (stand-alone kernels) and denoiser.cu (the fused decoder-layer kernel).  sm_90a only.
+// wgmma / TMA / mbarrier PTX wrappers and the fused feed-forward block as a device function, used by the kernels of
+// gemm_wgmma.cu.  sm_90a only.
 #pragma once
 #include "common.cuh"
 
@@ -143,7 +143,7 @@ __device__ __forceinline__ void split_kblock(float (&main)[NR], float (&small)[N
 // Then bias + residual, the layer's final LayerNorm, stores.
 //
 // Warp roles: warps 0-7 = two consumer warpgroups (rows 0-63 / 64-127 of the tile: wgmma, GELU, reduction), warp 8 = TMA
-// producer, warp 9 = exchange with the partner CTA; further warps of a larger CTA only take part in the barriers.
+// producer, warp 9 = exchange with the partner CTA.
 //
 // Shared memory (192 KB):  R0 [0, 64K)    GEMM 1 stage 0, then the partner's S (same layout as S)
 //                          R1 [64K, 128K) GEMM 1 stage 1, then the W2 ring: 2 slots of 32 KB (k-block of 64: hi 16K | lo 16K)
@@ -176,40 +176,37 @@ struct MlpArgs {
     float* Z; int ldz;
     const float *ln_w, *ln_b;
     __half *Zh, *Zl;
-    long long* trace;
 };
 
-// Barriers of the feed-forward block; ends with a CTA barrier.  The barrier words live ABOVE the 192 KB operand region, so
-// a caller may use that region for something else until mlp_run starts.
-// EARLY (stand-alone kernel: the operand region is free from the start): the thread that initialises the barriers also
-// requests the first two k-blocks of operands at once - W1 (step-invariant), then, after the dependency wait, X - instead of
-// leaving that to the producer warp after the CTA barrier.  mlp_run<true> then skips those requests.
-template <bool EARLY = false>
-__device__ __forceinline__ void mlp_setup(uint8_t* smem_raw, const MlpArgs& a, int j = 0, int m0 = 0) {
+// The feed-forward block of one 128-row tile on the cluster's 8 CTAs (see the comment above).  j = rank in the cluster =
+// hidden chunk; m0 = first row of the tile; rows >= M are neither reduced nor stored.  Called by all 320 threads of the CTA
+// (NUM_THREADS).
+__device__ __forceinline__ void mlp_tile(uint8_t* smem_raw, const MlpArgs& a, int j, int m0, int M, long long* tr) {
     using namespace mlp;
+    constexpr int NPASS = 1024 / (CW * 32);    // float4 elements of the 16 x 256 reduction slice per consumer thread
+#define MTRACE(slot) do { if (tr) tr[slot] = clock64(); } while (0)
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     const uint32_t bars = base + RING + S_BYTES;
     if (threadIdx.x == 0) {
-        if (EARLY) {
-            // the two "operands landed" barriers of GEMM 1 first, so that the first requests leave before the other barriers exist
-            mbar_init(bars, 1); mbar_init(bars + 8u, 1);
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-            for (int kb = 0; kb < 2; kb++) {
-                const uint32_t dst = base + kb * STAGE1;
-                mbar_arrive_expect_tx(bars + 8u * kb, STAGE1);
-                tma_load_2d(dst + 16384, a.map_w1, bars + 8u * kb, kb * BK, j * FC);
-                tma_load_2d(dst + 49152, a.map_w1l, bars + 8u * kb, kb * BK, j * FC);
-            }
-            pdl_wait();
-            chain_mark(2, 1);
-            for (int kb = 0; kb < 2; kb++) {
-                const uint32_t dst = base + kb * STAGE1;
-                tma_load_2d(dst, a.map_x, bars + 8u * kb, kb * BK, m0);
-                tma_load_2d(dst + 32768, a.map_xl, bars + 8u * kb, kb * BK, m0);
-            }
+        // The thread that initialises the barriers also requests the first two k-blocks of GEMM 1 at once - W1
+        // (step-invariant), then, after the dependency wait, X - before the CTA barrier.  The two "operands landed" barriers
+        // of GEMM 1 first, so that the first requests leave before the other barriers exist.
+        mbar_init(bars, 1); mbar_init(bars + 8u, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        for (int kb = 0; kb < 2; kb++) {
+            const uint32_t dst = base + kb * STAGE1;
+            mbar_arrive_expect_tx(bars + 8u * kb, STAGE1);
+            tma_load_2d(dst + 16384, a.map_w1, bars + 8u * kb, kb * BK, j * FC);
+            tma_load_2d(dst + 49152, a.map_w1l, bars + 8u * kb, kb * BK, j * FC);
+        }
+        pdl_wait();
+        chain_mark(2, 1);
+        for (int kb = 0; kb < 2; kb++) {
+            const uint32_t dst = base + kb * STAGE1;
+            tma_load_2d(dst, a.map_x, bars + 8u * kb, kb * BK, m0);
+            tma_load_2d(dst + 32768, a.map_xl, bars + 8u * kb, kb * BK, m0);
         }
         for (int s = 0; s < 2; s++) {
-            if (!EARLY) mbar_init(bars + 8u * s, 1);
             mbar_init(bars + 8u * (2 + s), CW); mbar_init(bars + 8u * (5 + s), 1); mbar_init(bars + 8u * (10 + s), CW);
             mbar_init(bars + 8u * (13 + s), 1); mbar_init(bars + 8u * (15 + s), 1);
         }
@@ -219,37 +216,19 @@ __device__ __forceinline__ void mlp_setup(uint8_t* smem_raw, const MlpArgs& a, i
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         // the partner's copies of its S k-blocks complete on these four (16 KB each: hi / lo of a k-block)
         for (int s = 0; s < 4; s++) mbar_arrive_expect_tx(bars + 8u * (13 + s), 16384u);
-        if (!EARLY) {
-            asm volatile("prefetch.tensormap [%0];" ::"l"(a.map_x) : "memory");
-            asm volatile("prefetch.tensormap [%0];" ::"l"(a.map_w1) : "memory");
-            asm volatile("prefetch.tensormap [%0];" ::"l"(a.map_xl) : "memory");
-            asm volatile("prefetch.tensormap [%0];" ::"l"(a.map_w1l) : "memory");
-        }
         asm volatile("prefetch.tensormap [%0];" ::"l"(a.map_w2) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(a.map_w2l) : "memory");
     }
     __syncthreads();
-}
 
-// The feed-forward block of one 128-row tile on the cluster's 8 CTAs (see the comment above).  j = rank in the cluster =
-// hidden chunk; m0 = first row of the tile; rows >= row_end are neither reduced nor stored (row_end <= M; a tile may hold
-// fewer than 128 live rows when the caller aligns tiles to samples).  wait_dep: execute griddepcontrol.wait before the first
-// dependent access (stand-alone launch); a caller that has already waited passes false.
-template <bool EARLY = false>
-__device__ __forceinline__ void mlp_run(uint8_t* smem_raw, const MlpArgs& a, int j, int m0, int row_end, bool wait_dep, long long* tr) {
-    using namespace mlp;
-    constexpr int NPASS = 1024 / (CW * 32);    // float4 elements of the 16 x 256 reduction slice per consumer thread
-#define MTRACE(slot) do { if (tr) tr[slot] = clock64(); } while (0)
     const CUtensorMap& map_x = *a.map_x; const CUtensorMap& map_w1 = *a.map_w1; const CUtensorMap& map_xl = *a.map_xl;
     const CUtensorMap& map_w1l = *a.map_w1l; const CUtensorMap& map_w2 = *a.map_w2; const CUtensorMap& map_w2l = *a.map_w2l;
     const float* __restrict__ b1 = a.b1; const float* __restrict__ b2 = a.b2; const float* __restrict__ res = a.res;
-    const int ldr = a.ldr, ldz = a.ldz, M = row_end;
+    const int ldr = a.ldr, ldz = a.ldz;
     float* __restrict__ Z = a.Z; const float* __restrict__ ln_w = a.ln_w; const float* __restrict__ ln_b = a.ln_b;
     __half* __restrict__ Zh = a.Zh; __half* __restrict__ Zl = a.Zl;
-    const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
     const uint32_t s_base = base + RING;
-    const uint32_t bars = base + RING + S_BYTES;
     auto bar_full1 = [&](int s) { return bars + 8u * s; };
     auto bar_empty1 = [&](int s) { return bars + 8u * (2 + s); };
     const uint32_t bar_g1done = bars + 8u * 4;
@@ -263,31 +242,10 @@ __device__ __forceinline__ void mlp_run(uint8_t* smem_raw, const MlpArgs& a, int
     const bool consumer = warp < CW;
     if (threadIdx.x == 0) MTRACE(1);
 
-    if (warp == CW && !EARLY) {
-        // ===================== TMA producer, first pipeline fill (EARLY: mlp_setup has already requested it) =====================
-        if (elect_one()) {
-            for (int kb = 0; kb < 2; kb++) {       // weight tiles do not depend on the previous kernel
-                const uint32_t dst = base + kb * STAGE1;
-                mbar_arrive_expect_tx(bar_full1(kb), STAGE1);
-                tma_load_2d(dst + 16384, &map_w1, bar_full1(kb), kb * BK, j * FC);
-                tma_load_2d(dst + 49152, &map_w1l, bar_full1(kb), kb * BK, j * FC);
-            }
-        }
-        __syncwarp();
-        if (wait_dep) { pdl_wait(); if (lane == 0) chain_mark(2, 1); }
-        if (elect_one()) {
-            for (int kb = 0; kb < 2; kb++) {
-                const uint32_t dst = base + kb * STAGE1;
-                tma_load_2d(dst, &map_x, bar_full1(kb), kb * BK, m0);
-                tma_load_2d(dst + 32768, &map_xl, bar_full1(kb), kb * BK, m0);
-            }
-        }
-        __syncwarp();
-    }
-    // Every CTA's barriers must exist (mlp_setup) before a partner arrives on them or copies into this CTA's shared memory:
+    // Every CTA's barriers must exist (above) before a partner arrives on them or copies into this CTA's shared memory:
     // one cluster barrier, arrive here, wait where each role first needs it (the consumers only after GEMM 1), so that its
     // latency stays off the critical path.
-    asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory");      // (mlp_setup's fence.mbarrier_init is the release)
+    asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory");      // (the fence.mbarrier_init above is the release)
 #define CLUSTER_WAIT() asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory")
 
     float4 o[NPASS];                     // this thread's elements of the closing reduction (consumers)
@@ -346,7 +304,7 @@ __device__ __forceinline__ void mlp_run(uint8_t* smem_raw, const MlpArgs& a, int
             }
             __syncwarp();
         }
-    } else if (consumer) {
+    } else {
         // ===================== consumer warpgroups =====================
         const int wg = warp >> 2;                                    // rows 64 wg .. of the tile
         const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);      // this thread's accumulator rows: r0 and r0 + 8
@@ -370,7 +328,7 @@ __device__ __forceinline__ void mlp_run(uint8_t* smem_raw, const MlpArgs& a, int
             }
             if (threadIdx.x == 0) MTRACE(3);
             CLUSTER_WAIT();
-            if (wait_dep) pdl_wait();
+            pdl_wait();
             // ---- bias + GELU -> (hi, lo) fp16 pairs in the swizzled K-major A layout, one k-block of S (64 hidden columns) at a
             // time, so that GEMM 2 and the copy to the partner can start on the first while the second is produced
 #pragma unroll
@@ -432,8 +390,6 @@ __device__ __forceinline__ void mlp_run(uint8_t* smem_raw, const MlpArgs& a, int
                                     fmaf(accs[4 * jx + 2 * hh + 1], 1.0f / 2048.0f, acc[4 * jx + 2 * hh + 1]));
             if (threadIdx.x == 0) MTRACE(9);
         }
-    } else {
-        CLUSTER_WAIT();
     }
 #undef CLUSTER_WAIT
     // ===================== cross-CTA reduction over distributed shared memory =====================
@@ -467,7 +423,6 @@ __device__ __forceinline__ void mlp_run(uint8_t* smem_raw, const MlpArgs& a, int
             o[t] = make_float4(0.f, 0.f, 0.f, 0.f);
             if (row < M) {
                 const float4 bb = *reinterpret_cast<const float4*>(b2 + c4 * 4);
-                // L2 read: in the fused layer kernel these rows were written by other CTAs of this launch
                 const float4 r4 = __ldcg(reinterpret_cast<const float4*>(res + (size_t)row * ldr + c4 * 4));
                 o[t] = make_float4((acc.x + bb.x) + r4.x, (acc.y + bb.y) + r4.y, (acc.z + bb.z) + r4.z, (acc.w + bb.w) + r4.w);
             }

@@ -95,7 +95,9 @@ class Engine:
         self._chk(self.lib.idb_debug_set_gemm_multicast(self._h, 1 if on else 0))
 
     def set_fused_mlp(self, on):
-        """Feed-forward block as one cluster kernel (default on) vs two GEMM launches."""
+        """Launch structure of the decoder layers.  2 (default): feed-forward block and the layer's final norm as one cluster
+        kernel; 0: the two GEMM launches.  10 / 11: self- and cross-attention of the standard layers as two launches / one
+        launch (default 11; identical results).  Other values raise EngineError and change nothing."""
         self._chk(self.lib.idb_set_fused_mlp(self._h, int(on)))
 
     def mlp(self, x, w1, b1, w2, b2, res, iters=1, trace=None, ln_w=None, ln_b=None):

@@ -18,7 +18,7 @@ from interdiff_b200.weights import bench_weights  # noqa: E402
 B = int(sys.argv[1]) if len(sys.argv) > 1 else 64
 steps = int(sys.argv[2]) if len(sys.argv) > 2 else 12
 mode = sys.argv[3] if len(sys.argv) > 3 else "loop"
-NAMES = {1: "gemm", 2: "mlp_fused", 3: "k_qan_xattn_ln", 4: "k_attn_ln", 5: "k_xattn_ln", 6: "k_step_io", 7: "k_layer_fused"}
+NAMES = {1: "gemm", 2: "mlp_fused", 3: "k_qan_xattn_ln", 4: "k_attn_ln", 5: "k_xattn_ln", 6: "k_step_io"}
 
 eng = Engine("cuda:0")
 eng.load_denoiser(bench_weights("diffusion_smpl"), "smpl")

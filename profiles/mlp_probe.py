@@ -31,7 +31,7 @@ eng.init_diffusion(get_named_beta_schedule("cosine", 100))
 tape = torch.from_numpy(S.noise_tape(b["gt"].shape, 100)).cuda()
 gt, mask = torch.from_numpy(b["gt"]).cuda(), torch.from_numpy(b["mask"]).cuda()
 outs = {}
-for on in (0, 1, 2, 1, 2):
+for on in (0, 2, 0, 2):
     eng.set_fused_mlp(on)
     for _ in range(2):
         out = eng.p_sample_loop(tape, gt, mask)
@@ -45,5 +45,5 @@ for on in (0, 1, 2, 1, 2):
     ms = e0.elapsed_time(e1) / 5
     outs[on] = out.clone()
     print("fused mlp %d: %.3f ms / 100 steps -> %.1f steps/s" % (on, ms, 100e3 / ms))
-print("max-norm rel diff of the 100-step samples between two GEMMs and the fused kernel: %.3e; with / without the fused norm: %.3e" % (
-    ((outs[0] - outs[1]).abs().max() / outs[0].abs().max()).item(), ((outs[2] - outs[1]).abs().max() / outs[1].abs().max()).item()))
+print("max-norm rel diff of the 100-step samples between two GEMMs and the fused kernel: %.3e" % (
+    ((outs[0] - outs[2]).abs().max() / outs[0].abs().max()).item()))

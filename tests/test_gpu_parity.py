@@ -393,9 +393,10 @@ def test_full_size_properties(eng):
 
 
 @pytest.mark.parametrize("M", [1920, 129])
-def test_fused_feed_forward_with_final_norm(eng, M):
+def test_fused_feed_forward_final_norm_and_two_gemms(eng, M):
     """level 2 of the fused feed-forward kernel: the layer's final LayerNorm applied in the reduction epilogue (two
-    named barriers across the 256 reducing threads), against float64 - and a whole forward with it switched on."""
+    named barriers across the 256 reducing threads), against float64 - and a whole forward with it switched on (level 2)
+    and off (level 0, the two GEMMs)."""
     g = torch.Generator().manual_seed(M + 1)
     x = torch.randn(M, 256, generator=g)
     w1 = torch.randn(1024, 256, generator=g) / 16
@@ -416,27 +417,33 @@ def test_fused_feed_forward_with_final_norm(eng, M):
     t = torch.tensor([900, 400, 50, 0])
     with torch.no_grad():
         ref_out = R.mdm_smpl_forward(sd, xx, t, torch.from_numpy(b["cond"]), faithful=False)
-    outs = {}
-    for level in (1, 2, 3):    # 1 = feed-forward only (the norm stays with the next kernel), 2 = default, 3 = whole layer in one launch
+    for level in (0, 2):    # 0 = the two GEMMs (the norm stays with the next kernel), 2 = default
         eng.set_fused_mlp(level)
-        outs[level] = eng.forward(xx.cuda(), t.cuda()).cpu()
-        assert rel(outs[level], ref_out) < 2e-4, level
+        out = eng.forward(xx.cuda(), t.cuda()).cpu()
+        assert rel(out, ref_out) < 2e-4, level
     eng.set_fused_mlp(2)
-    if M == 1920:
-        # level 3 (attention + feed-forward of a layer in ONE cluster kernel on sample-aligned 4-sample tiles) computes every
-        # row exactly like level 2: bit-identical, also with a partial last cluster (B = 7) and a 3-slab window (T = 35)
-        assert torch.equal(outs[3], outs[2])
-        for B2, T2 in ((7, 30), (3, 35), (9, 16)):
-            b2 = S.make_smpl_batch(B=B2, T=T2)
-            eng.bind(b2["cond"], T2)
-            x2 = torch.from_numpy(S.noise_tape(b2["gt"].shape, 0)[0]).cuda()
-            t2 = torch.randint(0, 1000, (B2,), generator=torch.Generator().manual_seed(B2)).cuda()
-            o = {}
-            for level in (2, 3):
-                eng.set_fused_mlp(level)
-                o[level] = eng.forward(x2, t2).clone()
-            eng.set_fused_mlp(2)
-            assert torch.equal(o[2], o[3]), (B2, T2)
+
+
+def test_fused_mlp_rejects_other_levels(eng):
+    """idb_set_fused_mlp accepts 0, 2, 10 and 11 only; any other value is an argument error that leaves the launch structure
+    as it was (the forward after it is bit-identical to the one before)."""
+    from interdiff_b200.engine import EngineError
+    sd = mdm_weights("smpl", "auto")
+    eng.load_denoiser(sd, "smpl")
+    b = S.make_smpl_batch(B=4, T=30)
+    eng.bind(b["cond"], 30)
+    x = torch.from_numpy(S.noise_tape(b["gt"].shape, 0)[0]).cuda()
+    t = torch.tensor([900, 400, 50, 0]).cuda()
+    eng.set_fused_mlp(10)          # start from the non-default state of both switches
+    eng.set_fused_mlp(0)
+    before = eng.forward(x, t).clone()
+    for bad in (1, 3, -1):
+        with pytest.raises(EngineError):
+            eng.set_fused_mlp(bad)
+    after = eng.forward(x, t).clone()
+    eng.set_fused_mlp(2)
+    eng.set_fused_mlp(11)
+    assert torch.equal(before, after)
 
 
 def test_launch_structure_switches_bit_identical(eng):
