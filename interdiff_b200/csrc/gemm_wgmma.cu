@@ -264,7 +264,7 @@ int make_map(idb_handle* h, CUtensorMap* map, const __half* ptr, int rows, int c
 
 CHAIN_SETTER(idb_chain_set_gemm)
 long long* g_idb_gemm_trace = nullptr;   // set by the debug hooks for ONE following launch
-int g_idb_gemm_wide_tiles = 1;           // 128-column tiles where they fill the SMs; 0 = 64-column tiles everywhere (test hook)
+int g_idb_gemm_wide_tiles = 1;           // 128-column tiles where idb_gemm_wgmma picks them; 0 = 64-column tiles everywhere (test hook)
 int g_idb_gemm_promote = 0;              // 0 = default; test hook (idb_debug_set_gemm_accumulators)
 
 bool idb_gemm_wgmma_supported(const GemmArgs& g) {
@@ -288,11 +288,13 @@ int idb_gemm_wgmma(idb_handle* h, const GemmArgs& g, cudaStream_t st) {
         CUDA_TRY(h, cudaFuncSetAttribute(gemm_split_f16_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<128>::SMEM_BYTES));
         h->attr_mask |= 1u;
     }
-    // wide outputs take 128-column tiles; narrow ones 64 so more SMs get a tile.  A tile's width does not change any
-    // element's result (same operations in the same order), so the choice is free to follow the SM count.
+    // wide single-accumulator outputs take 128-column tiles; everything else 64, so more SMs get a tile.  With the per-k-block
+    // fp32 promotion the 128-column kernel holds three 64-float accumulator sets at its 168-register cap and spills inside
+    // the k-loop: on an H100 it ran the 1920 x 1536 x 256 attention-projection GEMM in 37 us against 29 us for 64-column
+    // tiles.  A tile's width does not change any element's result (same operations in the same order), so the choice is free.
     const int row_tiles = (M + BM - 1) / BM;
     const long tiles128 = (long)row_tiles * ((N + 127) / 128);
-    const bool wide = g_idb_gemm_wide_tiles && 2 * tiles128 >= h->sm_count;
+    const bool wide = g_idb_gemm_wide_tiles && g.single_acc && 2 * tiles128 >= h->sm_count;
     CUtensorMap ma, mw, mal, mwl;
     int rc;
     if ((rc = make_map(h, &ma, g.A_hi, M, K, g.lda, BM))) return rc;
@@ -313,7 +315,7 @@ int idb_gemm_wgmma(idb_handle* h, const GemmArgs& g, cudaStream_t st) {
     // result does not depend on how many samples share the batch (multi-GPU runs slice one global batch; SURVEY 8e).
     int promote = g.single_acc ? (1 << 30) : 1;
     if (g_idb_gemm_promote > 0) promote = g_idb_gemm_promote;
-    if (wide && g.single_acc && h->gemm_multicast && row_tiles >= 2 && ksplit == 1 && !zero) {
+    if (wide && h->gemm_multicast && row_tiles >= 2 && ksplit == 1 && !zero) {
         // long, wide GEMMs (the SMPL-H blend): pairs of row tiles share the W tile by TMA multicast (cluster 1 x 2 x 1)
         if ((rc = make_map(h, &mw, g.W_hi, N, K, g.ldw, 64))) return rc;
         if ((rc = make_map(h, &mwl, g.W_lo, N, K, g.ldw, 64))) return rc;

@@ -148,7 +148,7 @@ __device__ __forceinline__ void split_kblock(float (&main)[NR], float (&small)[N
 // Shared memory (192 KB):  R0 [0, 64K)    GEMM 1 stage 0, then the partner's S (same layout as S)
 //                          R1 [64K, 128K) GEMM 1 stage 1, then the W2 ring: 2 slots of 32 KB (k-block of 64: hi 16K | lo 16K)
 //                          S  [128K,192K) S_hi [2][16K] | S_lo [2][16K]
-//                          after GEMM 2: the fp32 partial tile [128][132] at offset 0.
+//                          after GEMM 2: the fp32 partial tile [128][136] at offset 0.
 namespace mlp {
 constexpr int FC = 128;                       // hidden columns per CTA
 constexpr int CLUSTER = 8;                    // d_ff / FC
@@ -158,7 +158,8 @@ constexpr int STAGE1 = 64 * 1024;             // A_hi 16K | W1_hi 16K | A_lo 16K
 constexpr int RING = 2 * STAGE1;
 constexpr int S_BYTES = 64 * 1024;            // S_hi [2][16K] | S_lo [2][16K]
 constexpr int W2SLOT = 32 * 1024;             // W2 k-block: hi [128 rows][128 B] | lo
-constexpr int PLD = NH + 4;                   // fp32 partial row stride (floats)
+constexpr int PLD = NH + 8;                   // fp32 partial row stride (floats): a half-warp's float2 stores (4 rows x 8
+                                              // columns) fall on 32 distinct banks
 constexpr int SMEM_BYTES = RING + S_BYTES + 1024 /*alignment slack*/ + 1024 /*barriers*/;
 constexpr int CW = 8;                         // consumer warps
 // barriers (8 B each, above the operand region): full1[2] 0,1 | empty1[2] 2,3 | gemm1_done 4 | w2full[2] 5,6 | s_ready[0] 7 |
