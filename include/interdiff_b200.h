@@ -225,11 +225,27 @@ int idb_add_offset(idb_handle* h, int T, int B, int K, long long ld, int col0, f
 /* bisecting hook: 0 = the SMPL-H blend GEMM without TMA-multicast row-tile pairs (identical results; default 1) */
 int idb_debug_set_gemm_multicast(idb_handle* h, int on);
 
-/* ---- kernel-level hook (tests / bench roofline leg) -----------------------------------------
- * C[M,N] = epi(A[M,K] . W[N,K]^T) with the handle's GEMM backend; epi bit 0 bias, 1 GELU(erf),
- * 2 residual add, 3 SiLU (the fused epilogues of the nn.Linear calls of the denoiser). */
-int idb_debug_gemm(idb_handle* h, const float* A, const float* W, const float* bias, const float* res, float* C,
-                   int M, int N, int K, int epi, void* stream);
+/* ---- kernel-level hooks (tests / bench roofline leg) ----------------------------------------
+ * C[M,N] = epi(A[M,K] . W[N,K]^T) with the handle's GEMM backend, row-major with the given row strides (elements).
+ * epi bit 0 bias, 1 GELU(erf), 2 residual add, 3 SiLU (the fused epilogues of the nn.Linear calls of the denoiser);
+ * bit 6: tensor path, hi x hi products only (the lo terms dropped; throughput probe, not a result).
+ * An operand is fp32 (A / W) or an fp16 (hi, lo) pair (A_hi, A_lo / W_hi, W_lo: x = hi + lo 2^-11); the output is fp32 (C)
+ * and/or such a pair (C_hi, C_lo, row stride ldc).  ksplit 2: tensor path's split-K, reduced onto a C that is already zero.
+ * zero != NULL: rows [0, M) x columns [0, zero_cols) of that matrix (row stride zero_ld) are set to 0 as a side job.
+ * single_acc 1: one tensor-core accumulator over the whole K (no fp32 promotion per k-block; 128-column tiles when they fill
+ * the GPU).  pdl 1: programmatic dependent launch (pre-split weights only).  trace != NULL: per-CTA clock64 timeline
+ * [ctas][16] of a tensor-path launch (slot 0 is written by every CTA at entry). */
+typedef struct {
+    const float* A; const void* A_hi; const void* A_lo; int lda;
+    const float* W; const void* W_hi; const void* W_lo; int ldw;
+    const float* bias; const float* res; int ldr;
+    float* C; void* C_hi; void* C_lo; int ldc;
+    int M, N, K, epi;
+    float* zero; int zero_ld, zero_cols;
+    int ksplit, single_acc, pdl;
+    long long* trace;
+} idb_gemm_desc;
+int idb_debug_gemm_ex(idb_handle* h, const idb_gemm_desc* d, void* stream);
 /* the same launch repeated `iters` times from C (roofline leg: host overhead per launch stays small) */
 int idb_debug_gemm_repeat(idb_handle* h, const float* A, const float* W, const float* bias, const float* res, float* C,
                           int M, int N, int K, int epi, int iters, void* stream);
@@ -238,18 +254,17 @@ int idb_debug_gemm_repeat(idb_handle* h, const float* A, const float* W, const f
 int idb_debug_set_gemm_accumulators(int n);
 /* out[M][256] = [LayerNorm(] gelu(x w1^T + b1) w2^T + b2 + res [)] through the fused feed-forward kernel (fp32 device
    pointers; ln_w / ln_b NULL = no norm); iters > 1: launches 2..iters are timed (idb_debug_last_ms); trace != NULL:
-   clock64 timeline [ctas][16] of launch 1 */
+   clock64 timeline [ctas][16] of launch 1; out_hi / out_lo != NULL: the output's fp16 (hi, lo) pairs as well.  Rows >= M
+   of the outputs are not written. */
 int idb_debug_mlp(idb_handle* h, const float* x, const float* w1, const float* b1, const float* w2, const float* b2,
                   const float* res, float* out, int M, int iters, long long* trace, const float* ln_w, const float* ln_b,
-                  void* stream);
+                  void* out_hi, void* out_lo, void* stream);
 double idb_debug_last_ms(const idb_handle* h);
 /* clock64 phase timeline (16 slots, host pointer) of CTA (0,0) of the last fused QaN + cross-attention kernel */
 int idb_debug_attn_trace(long long* out16);
 /* chain timeline probe (profiles/chain_probe.py): device buffer of 64 lanes x (2 + 2 * capacity) uint64, lane[0] = 0, lane[1] = capacity; every
    kernel of the sampling step then appends (kind | event | grid | block, %globaltimer) records; NULL switches it off */
 int idb_debug_chain_trace(idb_handle* h, unsigned long long* buf);
-/* one launch with a per-CTA clock64 timeline (16 slots per CTA) of the wgmma kernel's pipeline */
-int idb_debug_gemm_trace(idb_handle* h, const float* A, const float* W, float* C, int M, int N, int K, long long* trace, void* stream);
 
 /* debug: fp16 (hi, lo) operand split (x = hi + lo * 2^-11), and a GEMM on such pairs */
 int idb_debug_split(idb_handle* h, const float* x, void* hi, void* lo, int rows, int cols, int ld_dst, void* stream);

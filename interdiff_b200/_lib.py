@@ -17,6 +17,18 @@ class DenoiserConfig(C.Structure):
                 ("rotary_offsets", C.c_float * 3)]
 
 
+class GemmDesc(C.Structure):
+    """idb_gemm_desc: one GEMM with every GemmArgs field a library caller sets (idb_debug_gemm_ex)."""
+    _fields_ = [("A", C.c_void_p), ("A_hi", C.c_void_p), ("A_lo", C.c_void_p), ("lda", C.c_int),
+                ("W", C.c_void_p), ("W_hi", C.c_void_p), ("W_lo", C.c_void_p), ("ldw", C.c_int),
+                ("bias", C.c_void_p), ("res", C.c_void_p), ("ldr", C.c_int),
+                ("C", C.c_void_p), ("C_hi", C.c_void_p), ("C_lo", C.c_void_p), ("ldc", C.c_int),
+                ("M", C.c_int), ("N", C.c_int), ("K", C.c_int), ("epi", C.c_int),
+                ("zero", C.c_void_p), ("zero_ld", C.c_int), ("zero_cols", C.c_int),
+                ("ksplit", C.c_int), ("single_acc", C.c_int), ("pdl", C.c_int),
+                ("trace", C.c_void_p)]
+
+
 _P = C.c_void_p
 _SIGS = {
     "idb_version": (C.c_int, []),
@@ -36,7 +48,7 @@ _SIGS = {
     "idb_set_dependent_launch": (C.c_int, [_P, C.c_int]),
     "idb_set_fused_mlp": (C.c_int, [_P, C.c_int]),
     "idb_set_nn_pruning": (C.c_int, [_P, C.c_int]),
-    "idb_debug_mlp": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P]),
+    "idb_debug_mlp": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P]),
     "idb_debug_last_ms": (C.c_double, [_P]),
     "idb_denoiser_init": (C.c_int, [_P, C.POINTER(DenoiserConfig)]),
     "idb_denoiser_load": (C.c_int, [_P, C.c_char_p, _P, C.POINTER(C.c_int64), C.c_int]),
@@ -61,14 +73,13 @@ _SIGS = {
     "idb_projector_set_hand_markers": (C.c_int, [_P, _P, C.c_int]),
     "idb_projector_sample": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P]),
     "idb_correction_bind": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, C.c_int, _P]),
-    "idb_debug_gemm": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
+    "idb_debug_gemm_ex": (C.c_int, [_P, C.POINTER(GemmDesc), _P]),
     "idb_debug_gemm_repeat": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "idb_debug_set_gemm_accumulators": (C.c_int, [C.c_int]),
     "idb_debug_attn_trace": (C.c_int, [C.POINTER(C.c_longlong)]),
     "idb_debug_split": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P]),
     "idb_debug_gemm_presplit": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "idb_debug_chain_trace": (C.c_int, [_P, _P]),
-    "idb_debug_gemm_trace": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
     "idb_correction_apply": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, _P, _P]),
     "idb_projector_init_skeleton": (C.c_int, [_P, C.c_int, C.c_int, C.c_int]),
     "idb_projector_sample_skeleton": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P]),

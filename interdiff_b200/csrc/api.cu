@@ -92,12 +92,13 @@ extern "C" int idb_set_fused_mlp(idb_handle* h, int on) {
 
 extern long long* g_idb_gemm_trace;
 /* test hook: out[M][256] = gelu(x w1^T + b1) w2^T + b2 + res through the fused cluster kernel (fp32 device inputs,
-   x [M][256], w1 [1024][256], w2 [256][1024]); operands are split into fp16 pairs in temporary buffers */
+   x [M][256], w1 [1024][256], w2 [256][1024]); operands are split into fp16 pairs in temporary buffers.  out_hi / out_lo
+   (NULL = none): the output's fp16 (hi, lo) pairs, row stride 256 like out.  Only rows < M of the outputs are written. */
 extern "C" int idb_debug_mlp(idb_handle* h, const float* x, const float* w1, const float* b1, const float* w2, const float* b2,
                              const float* res, float* out, int M, int iters, long long* trace, const float* ln_w, const float* ln_b,
-                             void* stream) {
+                             void* out_hi, void* out_lo, void* stream) {
     IDB_ENTER(h);
-    if (!h || !x || !w1 || !b1 || !w2 || !b2 || !res || !out || M <= 0) return IDB_ERR_ARG;
+    if (!h || !x || !w1 || !b1 || !w2 || !b2 || !res || !out || M <= 0 || (out_hi == nullptr) != (out_lo == nullptr)) return IDB_ERR_ARG;
     cudaStream_t st = (cudaStream_t)stream;
     const int Dm = 256, F = 1024;
     __half* buf = nullptr;
@@ -112,8 +113,9 @@ extern "C" int idb_debug_mlp(idb_handle* h, const float* x, const float* w1, con
     for (int i = 0; i < (iters > 0 ? iters : 1) && !rc; i++) {
         if (i == 0 && trace) g_idb_gemm_trace = trace;
         if (i == 1) cudaEventRecord(e0, st);
-        rc = idb_mlp_wgmma(h, xh, xl, w1h, w1l, b1, w2h, w2l, b2, res, Dm, out, Dm, M, 0, st, ln_w, ln_b, nullptr, nullptr);
+        rc = idb_mlp_wgmma(h, xh, xl, w1h, w1l, b1, w2h, w2l, b2, res, Dm, out, Dm, M, 0, st, ln_w, ln_b, (__half*)out_hi, (__half*)out_lo);
     }
+    g_idb_gemm_trace = nullptr;
     cudaEventRecord(e1, st);
     cudaStreamSynchronize(st);
     if (iters > 1 && !rc) { float ms = 0.f; cudaEventElapsedTime(&ms, e0, e1); h->last_ms = ms / (iters - 1); }
@@ -122,19 +124,23 @@ extern "C" int idb_debug_mlp(idb_handle* h, const float* x, const float* w1, con
     return rc;
 }
 
-extern "C" int idb_debug_gemm(idb_handle* h, const float* A, const float* W, const float* bias, const float* res, float* C,
-                              int M, int N, int K, int epi, void* stream) {
+/* test hook: one GEMM with every GemmArgs field a library caller sets (the tensor path's split-K onto a C the caller zeroed,
+   the aux-zero side job, fp16 (hi, lo) operands and outputs, strides, single accumulator, dependent launch) */
+extern "C" int idb_debug_gemm_ex(idb_handle* h, const idb_gemm_desc* d, void* stream) {
     IDB_ENTER(h);
-    if (!h || !A || !W || !C) return IDB_ERR_ARG;
-    if (epi & 128) {   /* test hook: split-K = 2 onto a C zeroed here */
-        cudaStream_t st = (cudaStream_t)stream;
-        CUDA_TRY(h, cudaMemsetAsync(C, 0, sizeof(float) * (size_t)M * N, st));
-        GemmArgs g;
-        g.A = A; g.lda = K; g.W = W; g.ldw = K; g.bias = bias; g.res = res; g.ldr = N; g.C = C; g.ldc = N;
-        g.M = M; g.N = N; g.K = K; g.epi = epi & ~128; g.ksplit = 2;
-        return idb_gemm_ex(h, g, st);
-    }
-    return idb_gemm(h, A, K, W, K, bias, res, N, C, N, M, N, K, epi, (cudaStream_t)stream);
+    if (!h || !d) return IDB_ERR_ARG;
+    GemmArgs g;
+    g.A = d->A; g.A_hi = (const __half*)d->A_hi; g.A_lo = (const __half*)d->A_lo; g.lda = d->lda;
+    g.W = d->W; g.W_hi = (const __half*)d->W_hi; g.W_lo = (const __half*)d->W_lo; g.ldw = d->ldw;
+    g.bias = d->bias; g.res = d->res; g.ldr = d->ldr;
+    g.C = d->C; g.C_hi = (__half*)d->C_hi; g.C_lo = (__half*)d->C_lo; g.ldc = d->ldc;
+    g.M = d->M; g.N = d->N; g.K = d->K; g.epi = d->epi;
+    g.ksplit = d->ksplit; g.zero = d->zero; g.zero_ld = d->zero_ld; g.zero_cols = d->zero_cols;
+    g.pdl = d->pdl; g.single_acc = d->single_acc;
+    g_idb_gemm_trace = d->trace;
+    const int rc = idb_gemm_ex(h, g, (cudaStream_t)stream);
+    g_idb_gemm_trace = nullptr;     // not consumed when the call took the SIMT path or failed before the launch
+    return rc;
 }
 
 /* same GEMM launched `iters` times back to back from C (keeps host overhead per launch small) */
@@ -149,7 +155,6 @@ extern "C" int idb_debug_gemm_repeat(idb_handle* h, const float* A, const float*
     return IDB_OK;
 }
 
-extern long long* g_idb_gemm_trace;
 static int g_idb_trace_epi = 0;
 int idb_chain_set_gemm(unsigned long long* buf);
 int idb_chain_set_denoiser(unsigned long long* buf);
@@ -159,20 +164,12 @@ extern "C" int idb_debug_chain_trace(idb_handle* h, unsigned long long* buf) {
     if (!h) return IDB_ERR_ARG;
     return (idb_chain_set_gemm(buf) | idb_chain_set_denoiser(buf)) ? IDB_ERR_CUDA : IDB_OK;
 }
-/* one GEMM launch with a per-CTA clock64 timeline written to trace[ctas][16] (device) */
-extern "C" int idb_debug_gemm_trace(idb_handle* h, const float* A, const float* W, float* C, int M, int N, int K, long long* trace, void* stream) {
-    IDB_ENTER(h);
-    if (!h || !A || !W || !C || !trace) return IDB_ERR_ARG;
-    g_idb_gemm_trace = trace;
-    return idb_gemm(h, A, K, W, K, nullptr, nullptr, N, C, N, M, N, K, g_idb_trace_epi, (cudaStream_t)stream);
-}
-
 extern int g_idb_gemm_promote;
 extern int g_idb_gemm_wide_tiles;
 /* test hook: k-blocks the big x big products accumulate in the tensor core between fp32 promotions (0 = default); 900 / 901: 128-column tiles off / on */
 extern "C" int idb_debug_set_gemm_accumulators(int n) {
     if (n == 900 || n == 901) { g_idb_gemm_wide_tiles = n - 900; return IDB_OK; }
-    if (n >= 1000) { g_idb_trace_epi = n - 1000; return IDB_OK; }   // >= 1000: epi flags for idb_debug_gemm_trace
+    if (n >= 1000) { g_idb_trace_epi = n - 1000; return IDB_OK; }   // >= 1000: epi flags for idb_debug_gemm_presplit
     g_idb_gemm_promote = n;
     return IDB_OK;
 }

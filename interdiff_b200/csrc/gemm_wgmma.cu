@@ -3,8 +3,11 @@
 // Why split precision: the sampling chain amplifies operand rounding (DESIGN.md "Conditioning"),
 // so the tensor-core path has to be fp32-grade.  Every fp32 operand x is carried as a pair of fp16
 //     hi = fp16_rn(x),   lo = fp16_rn((x - hi) * 2^11)          (x - hi is exact in fp32)
-// so that x = hi + lo * 2^-11 up to 2^-23 |x| (the 2^11 scale keeps `lo` a normal fp16 number), and
+// so that x = hi + lo * 2^-11 up to max(2^-23 |x|, 2^-36), and
 //     A W^T = A_hi W_hi^T  +  2^-11 (A_lo W_hi^T + A_hi W_lo^T)  (+ 2^-22 A_lo W_lo^T, dropped).
+// The 2^11 scale keeps `lo` a normal fp16 number while |x - hi| >= 2^-25; below that lo is subnormal (spacing 2^-24, i.e.
+// 2^-35 in units of x), so the relative 2^-23 holds for |x| >= 2^-13 and smaller operands carry an absolute error of at
+// most 2^-36 (for |x| < 2^-14 hi itself is subnormal).  tests/test_gpu_gemm_kernels.py checks this floor element by element.
 // The two sums accumulate in SEPARATE fp32 register accumulators and are combined in the epilogue.
 // Range: |x| < 65504 (activations and weights of this model are O(1e-3 .. 1e3)).
 //

@@ -100,16 +100,25 @@ class Engine:
         launch (default 11; identical results).  Other values raise EngineError and change nothing."""
         self._chk(self.lib.idb_set_fused_mlp(self._h, int(on)))
 
-    def mlp(self, x, w1, b1, w2, b2, res, iters=1, trace=None, ln_w=None, ln_b=None):
-        """gelu(x @ w1.T + b1) @ w2.T + b2 + res through the fused feed-forward kernel (tests / probes).
-        iters > 1: self.last_ms() is the mean time of launches 2..iters; trace: int64 [ctas,16] device tensor."""
+    def mlp(self, x, w1, b1, w2, b2, res, iters=1, trace=None, ln_w=None, ln_b=None, *, out=None, out_pair=None):
+        """gelu(x @ w1.T + b1) @ w2.T + b2 + res [-> LayerNorm(ln_w, ln_b)] through the fused feed-forward kernel (tests / probes).
+        iters > 1: self.last_ms() is the mean time of launches 2..iters; trace: int64 [ctas,16] device tensor.
+        out: contiguous fp32 [>= M, 256] device tensor to write rows [0, M) of (rows past M are left as they are);
+        out_pair: (hi, lo) contiguous fp16 tensors of out's shape that receive the output's fp16 pairs too."""
         x, w1, b1, w2, b2, res = (self._f32(t) for t in (x, w1, b1, w2, b2, res))
-        out = torch.empty_like(x)
+        M = x.shape[0]
+        if out is None:
+            out = torch.empty_like(x)
+        ok = lambda t, dt: t.device == self.device and t.dtype == dt and t.is_contiguous() and t.dim() == 2 and t.shape[0] >= M \
+            and t.shape[1] == 256
+        if not ok(out, torch.float32) or (out_pair is not None and not all(ok(t, torch.float16) for t in out_pair)):
+            raise EngineError("mlp: outputs are contiguous [>= M, 256] device tensors (fp32 out, fp16 out_pair)")
         ln_w = self._f32(ln_w) if ln_w is not None else None
         ln_b = self._f32(ln_b) if ln_b is not None else None
+        zh, zl = out_pair if out_pair is not None else (None, None)
         self._chk(self.lib.idb_debug_mlp(self._h, self._ptr(x), self._ptr(w1), self._ptr(b1), self._ptr(w2), self._ptr(b2), self._ptr(res),
-                                         self._ptr(out), x.shape[0], int(iters), self._ptr(trace), self._ptr(ln_w), self._ptr(ln_b),
-                                         self._stream()))
+                                         self._ptr(out), M, int(iters), self._ptr(trace), self._ptr(ln_w), self._ptr(ln_b),
+                                         self._ptr(zh), self._ptr(zl), self._stream()))
         return out
 
     def last_ms(self):
@@ -119,20 +128,69 @@ class Engine:
         self._chk(self.lib.idb_set_gemm_backend(self._h, {"simt": 0, "tcgen05": 1}.get(backend, backend)))
 
     # ------------------------------------------------------------------ kernel-level hooks
-    def gemm(self, A, W, bias=None, res=None, gelu=False, silu=False, split_k=False):
-        """epi(A @ W.T) through the handle's GEMM backend (tests / roofline leg).  split_k: the tensor path's
-        2-way split-K variant (two partial tiles reduced onto a zeroed C), as the denoiser runs ff2."""
-        A, W = self._f32(A), self._f32(W)
+    def _rows(self, t, dtype):
+        """A row-major device matrix of `dtype` with unit column stride, as given (a view of a wider buffer keeps its row
+        stride) or copied to the device."""
+        if isinstance(t, np.ndarray):
+            t = torch.from_numpy(t)
+        if not (t.device == self.device and t.dtype == dtype and t.dim() == 2 and t.stride(1) == 1):
+            t = t.to(device=self.device, dtype=dtype).contiguous()
+        return t
+
+    def _operand(self, t):
+        """fp32 matrix -> (t, None, None, ld); (hi, lo) fp16 pair -> (None, hi, lo, ld)"""
+        if isinstance(t, (tuple, list)):
+            hi, lo = (self._rows(x, torch.float16) for x in t)
+            if hi.shape != lo.shape or hi.stride() != lo.stride():
+                raise EngineError("an fp16 (hi, lo) operand needs two parts of one shape and row stride")
+            return None, hi, lo, hi.stride(0)
+        t = self._rows(t, torch.float32)
+        return t, None, None, t.stride(0)
+
+    def gemm(self, A, W, bias=None, res=None, gelu=False, silu=False, split_k=False, *, out=None, out_pair=None, zero=None,
+             single_acc=False, pdl=False, hi_only=False, trace=None):
+        """epi(A @ W.T) through the handle's GEMM backend (tests / roofline leg), via idb_debug_gemm_ex.
+        A, W: fp32 matrices or fp16 (hi, lo) pairs (x = hi + lo 2^-11, idb_debug_split); views of wider row-major buffers are
+        used in place, with their row stride, as are res, out and the out_pair parts.
+        split_k: the tensor path's 2-way split-K (two partial tiles reduced onto C), as the denoiser runs ff2; the result is
+        added to `out`, which must hold zeros (a new zeroed C when out is None).
+        out_pair: (hi, lo) fp16 matrices that receive the output as a pair too (same row stride as `out`); with out_pair and
+        no `out` only the pair is written (the kernel gets no fp32 output).
+        zero: a view [M, cols] of an fp32 matrix that the GEMM sets to zero as a side job.
+        single_acc: one tensor-core accumulator over the whole K (no per-k-block fp32 promotion).  pdl: programmatic dependent
+        launch (pre-split W).  hi_only: tensor path with the lo terms dropped (epi bit 64).  trace: int64 [ctas, 16] device
+        tensor for the per-CTA timeline.
+        Returns out, or out_pair when only the pair was requested."""
+        a, ah, al, lda = self._operand(A)
+        w, wh, wl, ldw = self._operand(W)
+        M, K = (a if a is not None else ah).shape
+        N = (w if w is not None else wh).shape[0]
         bias = self._f32(bias) if bias is not None else None
-        res = self._f32(res) if res is not None else None
-        M, K = A.shape
-        N = W.shape[0]
-        out = torch.empty(M, N, device=self.device)
-        epi = (1 if bias is not None else 0) | (2 if gelu else 0) | (4 if res is not None else 0) | (8 if silu else 0)
-        epi |= 128 if split_k else 0
-        self._chk(self.lib.idb_debug_gemm(self._h, self._ptr(A), self._ptr(W), self._ptr(bias), self._ptr(res), self._ptr(out),
-                                          M, N, K, epi, self._stream()))
-        return out
+        res = self._rows(res, torch.float32) if res is not None else None
+        if out is None and out_pair is None:
+            out = (torch.zeros if split_k else torch.empty)(M, N, device=self.device)
+        elif out is not None:
+            out = self._rows(out, torch.float32)
+        d = _lib.GemmDesc()
+        d.A, d.A_hi, d.A_lo, d.lda = self._ptr(a), self._ptr(ah), self._ptr(al), lda
+        d.W, d.W_hi, d.W_lo, d.ldw = self._ptr(w), self._ptr(wh), self._ptr(wl), ldw
+        d.bias, d.res, d.ldr = self._ptr(bias), self._ptr(res), res.stride(0) if res is not None else N
+        d.C, d.ldc = self._ptr(out), out.stride(0) if out is not None else N
+        if out_pair is not None:
+            ch, cl = out_pair
+            if not all(t.dtype == torch.float16 and t.device == self.device and t.stride(1) == 1 for t in (ch, cl)) or \
+                    ch.stride(0) != cl.stride(0) or (out is not None and ch.stride(0) != out.stride(0)):
+                raise EngineError("out_pair: two fp16 device matrices with the row stride of out")
+            d.C_hi, d.C_lo, d.ldc = self._ptr(ch), self._ptr(cl), ch.stride(0)
+        d.M, d.N, d.K = M, N, K
+        d.epi = (1 if bias is not None else 0) | (2 if gelu else 0) | (4 if res is not None else 0) | (8 if silu else 0) | (64 if hi_only else 0)
+        if zero is not None:
+            assert zero.dtype == torch.float32 and zero.device == self.device and zero.stride(1) == 1
+            d.zero, d.zero_ld, d.zero_cols = self._ptr(zero), zero.stride(0), zero.shape[1]
+        d.ksplit, d.single_acc, d.pdl = (2 if split_k else 1), int(bool(single_acc)), int(bool(pdl))
+        d.trace = self._ptr(trace)
+        self._chk(self.lib.idb_debug_gemm_ex(self._h, C.byref(d), self._stream()))
+        return out if out is not None else out_pair
 
     def gemm_microbench(self, M, N, K, iters=200, gelu=True, split_k=False):
         """Mean device time of one tensor-core GEMM launch (fp16-pair operands as the denoiser feeds them,

@@ -1,4 +1,4 @@
-"""GEMM backends of the C ABI (idb_debug_gemm) against a float64 reference.  The tcgen05 backend
+"""GEMM backends of the C ABI (idb_debug_gemm_ex through Engine.gemm) against a float64 reference.  The tcgen05 backend
 must be fp32-grade (split precision on fp16 (hi, lo) pairs): the bound asserted for it is the same as for the
 fp32 SIMT kernel, far below plain-TF32 error (~5e-4)."""
 import pytest
@@ -17,7 +17,7 @@ def eng():
 
 SHAPES = [(1920, 1024, 256), (1920, 256, 1024), (1920, 768, 256), (1920, 256, 256), (640, 512, 256),
           (100, 72, 36), (129, 200, 100), (1, 8, 4), (300, 1024, 260),
-          (1920, 1536, 256), (2500, 1280, 200)]   # more 128-column tiles than the H100 has SMs (132): several waves
+          (1920, 1536, 256), (2500, 1280, 200)]   # more 64-column tiles (360, 400) than an H100 has SMs: several waves
 
 
 @pytest.mark.parametrize("backend", ["simt", "tcgen05"])

@@ -448,9 +448,7 @@ def test_fused_mlp_rejects_other_levels(eng):
 
 def test_launch_structure_switches_bit_identical(eng):
     """The launch-structure options of the step compute every row with the same arithmetic: self- + cross-attention of the
-    standard layers as one launch vs two (idb_set_fused_mlp 11 / 10), 128- vs 64-column GEMM tiles
-    (idb_debug_set_gemm_accumulators 901 / 900; the hook keeps its name, other values set the fp32 promotion interval:
-    same operations in the same k order per element whatever the tile width)."""
+    standard layers as one launch vs two (idb_set_fused_mlp 11 / 10)."""
     sd = mdm_weights("smpl", "auto")
     eng.load_denoiser(sd, "smpl")
     for B2, T2 in ((64, 30), (5, 35), (9, 16)):
@@ -462,13 +460,7 @@ def test_launch_structure_switches_bit_identical(eng):
         eng.set_fused_mlp(10)
         two = eng.forward(x, t).clone()
         eng.set_fused_mlp(11)
-        eng.lib.idb_debug_set_gemm_accumulators(900)
-        eng.set_fused_mlp(2)          # (drops the captured graphs)
-        wide = eng.forward(x, t).clone()
-        eng.lib.idb_debug_set_gemm_accumulators(901)
-        eng.set_fused_mlp(2)
         assert torch.equal(base, two), (B2, T2)
-        assert torch.equal(base, wide), (B2, T2)
 
 
 def test_rotation_conversions_targeted(eng):

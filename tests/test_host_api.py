@@ -110,3 +110,25 @@ def test_skeleton_projector_mirror_loads_checkpoint_strictly():
     assert not missing and not unexpected
     from interdiff_b200 import weights as W2
     assert set(W2.projector_skeleton_shapes()) == {k for k in sd if "num_batches_tracked" not in k}
+
+
+def test_checkpoint_weights_against_the_precision_floor(record_property):
+    """The exported checkpoint's GEMM weights: entries below 2^-13 lose the 2^-23 relative precision of the pair
+    (absolute floor 2^-36).  Per weight row that adds at most K 2^-36 |x|, which must stay below one 2^-23 relative unit of
+    the row's l1 norm for O(1) activations."""
+    from interdiff_b200 import weights as Wt
+    found = False
+    for name in ("diffusion_smpl", "diffusion_smpl_encoder", "diffusion_skeleton"):
+        sd = Wt.load_ref_weights(name)
+        if sd is None:
+            continue
+        found = True
+        for k, w in sd.items():
+            if not k.endswith("weight") or w.ndim != 2 or "norm" in k:
+                continue
+            a = np.abs(w.astype(np.float64))
+            nz = a[a > 0]
+            record_property("min_abs_%s.%s" % (name, k), float(nz.min()) if nz.size else 0.0)
+            assert np.all(a.shape[1] * 2.0 ** -36 <= 2.0 ** -23 * a.sum(axis=1) + (a.sum(axis=1) == 0)), k
+    if not found:
+        pytest.skip("exported reference weights not present")
