@@ -166,9 +166,12 @@ extern "C" int idb_debug_chain_trace(idb_handle* h, unsigned long long* buf) {
 }
 extern int g_idb_gemm_promote;
 extern int g_idb_gemm_wide_tiles;
-/* test hook: k-blocks the big x big products accumulate in the tensor core between fp32 promotions (0 = default); 900 / 901: 128-column tiles off / on */
+extern int g_idb_gemm_persistent;
+/* test hook: k-blocks the big x big products accumulate in the tensor core between fp32 promotions (0 = default); 900 / 901: 128-column tiles off / on;
+   910 / 911: one tile per CTA / the persistent schedule (default) of the 64-column kernel */
 extern "C" int idb_debug_set_gemm_accumulators(int n) {
     if (n == 900 || n == 901) { g_idb_gemm_wide_tiles = n - 900; return IDB_OK; }
+    if (n == 910 || n == 911) { g_idb_gemm_persistent = n - 910; return IDB_OK; }
     if (n >= 1000) { g_idb_trace_epi = n - 1000; return IDB_OK; }   // >= 1000: epi flags for idb_debug_gemm_presplit
     g_idb_gemm_promote = n;
     return IDB_OK;

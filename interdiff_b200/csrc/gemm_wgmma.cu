@@ -11,14 +11,14 @@
 // The two sums accumulate in SEPARATE fp32 register accumulators and are combined in the epilogue.
 // Range: |x| < 65504 (activations and weights of this model are O(1e-3 .. 1e3)).
 //
-// Pipeline per CTA (one 128 x BN output tile, 288 threads):
+// Pipeline per CTA (128 x BN output tiles, 288 threads; the 64-column kernel is persistent, see gemm_split_f16_persistent):
 //   warp 8    : TMA producer (warp-uniform loop, one elected lane issues): 4 x cp.async.bulk.tensor.2d per
 //               stage (A_hi, W_hi, A_lo, W_lo k-blocks of 64 fp16 = one 128B-swizzle row), mbarrier tx.
 //   warps 0-7 : two consumer warpgroups, 64 rows of the tile each: 12 wgmma.mma_async m64nBNk16 per k-block
 //               (4 k-steps of 16 x {lo*hi, hi*lo -> small; hi*hi -> main}), release of the stage, then the
-//               epilogue straight from the accumulator registers: sum, bias / GELU / SiLU, residual, stores (a quad
-//               of lanes covers one 32-byte sector of a row); optional output already split into (hi, lo) fp16
-//               pairs for the next GEMM.
+//               epilogue: sum, bias / GELU / SiLU, residual, stores (128-column kernels: straight from the accumulator
+//               registers, a quad of lanes covers one 32-byte sector of a row; 64-column kernel: staged through shared
+//               memory, whole rows); optional output already split into (hi, lo) fp16 pairs for the next GEMM.
 // The tensor core truncates on every fp32 accumulate, so the hi*hi products of every k-block (or of `promote`
 // k-blocks) go into a fresh accumulator that is then added to the running sum with an IEEE fp32 addition.  The order
 // of the additions per output element is a function of K alone - not of the tile width or of M.
@@ -221,6 +221,227 @@ gemm_split_f16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_co
 #undef TRACE
 }
 
+// Persistent 64-column kernel (every GEMM that does not take the 128-column kernels above).  Grid (cpr, gy, ksplit), at most
+// one CTA per SM: CTA (x, y) owns the contiguous run of column tiles [x ct / cpr, (x + 1) ct / cpr) of row tiles y, y + gy, ..
+// (ct = column tiles).  The schedule is a function of the shape and the SM count only, and an element's additions are the
+// same whatever CTA computes its tile.
+// Shared memory: A ring of 4 slots of 32 KB (a k-block of the 128-row tile: hi 16 KB | lo 16 KB), W ring of 4 slots of 16 KB
+// (hi 8 KB | lo 8 KB), each with full / empty barriers.  When the CTA's k-blocks fit into the A ring (K <= 256 per split), a
+// row tile's A block is loaded once and stays resident across the CTA's column tiles, released after the last of them: A
+// traffic drops by the column tiles per CTA.  Otherwise A streams with W, one A slot per k-block.  The producer runs ahead
+// across tile boundaries, so the next tile's loads are in flight while the consumers run the epilogue.
+namespace pers {
+constexpr int A_SLOTS = 4, W_SLOTS = 4;
+constexpr int A_BYTES = 2 * BM * BK * 2;       // hi | lo
+constexpr int W_BYTES = 2 * 64 * BK * 2;       // hi | lo
+constexpr int W_OFF = A_SLOTS * A_BYTES;
+constexpr int E_OFF = W_OFF + W_SLOTS * W_BYTES;
+constexpr int E_BYTES = 16 * 64 * 4;           // a consumer warp's 16 x 64 fp32 rows of the tile, staged for the epilogue
+constexpr int SMEM_BYTES = E_OFF + GEMM_CW * E_BYTES + 1024 /*align*/ + 256 /*barriers*/;     // 224 KB + 1.25 KB
+}  // namespace pers
+
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_split_f16_persistent(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w,
+                          const __grid_constant__ CUtensorMap map_al, const __grid_constant__ CUtensorMap map_wl,
+                          const float* __restrict__ bias, const float* __restrict__ res, int ldr,
+                          float* __restrict__ C, __half* __restrict__ Ch, __half* __restrict__ Cl, int ldc, int M, int N, int K, int epi,
+                          int promote, float* __restrict__ zero_ptr, int zero_ld, int zero_cols, long long* __restrict__ trace) {
+    using namespace pers;
+    constexpr int BN = 64, NR = BN / 2;
+    const long long t_entry = clock64();
+    if (threadIdx.x == 0) chain_mark(1, 0);
+    pdl_trigger();   // the next kernel may start its own prologue now (it blocks in pdl_wait before touching our output)
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+    const uint32_t bars = base + E_OFF + GEMM_CW * E_BYTES;
+    // barriers (8 B each): a_full[4], a_empty[4], w_full[4], w_empty[4]
+    auto a_full = [&](int s) { return bars + 8u * s; };
+    auto a_empty = [&](int s) { return bars + 8u * (A_SLOTS + s); };
+    auto w_full = [&](int s) { return bars + 8u * (2 * A_SLOTS + s); };
+    auto w_empty = [&](int s) { return bars + 8u * (2 * A_SLOTS + W_SLOTS + s); };
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int ct = (N + BN - 1) / BN, rt = (M + BM - 1) / BM;
+    const int c_begin = blockIdx.x * ct / gridDim.x, ncols = (blockIdx.x + 1) * ct / gridDim.x - c_begin;
+    const int nrows = (rt - blockIdx.y + gridDim.y - 1) / gridDim.y;
+    // split-K: blockIdx.z owns a contiguous range of k-blocks; the partial tiles are combined with
+    // fp32 reductions onto a zeroed C (two addends only, so the result does not depend on their order)
+    const int total_kb = (K + BK - 1) / BK, per_kb = (total_kb + gridDim.z - 1) / gridDim.z;
+    const int kb0 = blockIdx.z * per_kb;
+    const int num_kb = min(per_kb, total_kb - kb0);
+    const bool resident = num_kb <= A_SLOTS;
+    const int total_w = nrows * ncols * num_kb;      // W k-blocks this CTA loads, in consumption order
+    // item i (one k-block of one tile) -> row tile, column tile
+    auto item_row = [&](int i) { return blockIdx.y + (i / num_kb / ncols) * gridDim.y; };
+    auto item_col = [&](int i) { return c_begin + (i / num_kb) % ncols; };
+    // optional per-tile timeline (clock64 at named points; profiles/gemm_trace.py lists the slots), one record per tile
+    auto rec = [&](int r, int c) { return trace ? trace + ((size_t)r * ct + c) * 16 : nullptr; };
+    long long* const tr_first = rec(blockIdx.y, c_begin);
+
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < A_SLOTS; s++) { mbar_init(a_full(s), 1); mbar_init(a_empty(s), GEMM_CW); }
+        for (int s = 0; s < W_SLOTS; s++) { mbar_init(w_full(s), 1); mbar_init(w_empty(s), GEMM_CW); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_al) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_wl) : "memory");
+    }
+    __syncthreads();
+    if (threadIdx.x == 0 && tr_first) { tr_first[0] = t_entry; tr_first[1] = clock64(); }
+
+    if (warp == GEMM_CW) {
+        // ===================== TMA producer =====================
+        auto load_w = [&](int i) {
+            const int s = i % W_SLOTS;
+            const uint32_t dst = base + W_OFF + s * W_BYTES;
+            const int k = (kb0 + i % num_kb) * BK, n0 = item_col(i) * BN;
+            mbar_arrive_expect_tx(w_full(s), W_BYTES);
+            tma_load_2d(dst, &map_w, w_full(s), k, n0);
+            tma_load_2d(dst + W_BYTES / 2, &map_wl, w_full(s), k, n0);
+        };
+        // The first W k-blocks do not depend on the previous kernel: requested before the dependency wait.
+        const int npre = min(total_w, W_SLOTS);
+        if (elect_one()) {
+            for (int i = 0; i < npre; i++) load_w(i);
+        }
+        __syncwarp();
+        pdl_wait();
+        if (lane == 0) chain_mark(1, 1);
+        int ai = 0;      // A k-blocks loaded so far
+        for (int i = 0; i < total_w; i++) {
+            if (!resident || item_col(i) == c_begin) {
+                const int s = ai % A_SLOTS;
+                if (ai >= A_SLOTS) mbar_wait(a_empty(s), (ai / A_SLOTS - 1) & 1);
+                if (elect_one()) {
+                    const uint32_t dst = base + s * A_BYTES;
+                    const int k = (kb0 + i % num_kb) * BK, m0 = item_row(i) * BM;
+                    mbar_arrive_expect_tx(a_full(s), A_BYTES);
+                    tma_load_2d(dst, &map_a, a_full(s), k, m0);
+                    tma_load_2d(dst + A_BYTES / 2, &map_al, a_full(s), k, m0);
+                }
+                __syncwarp();
+                ai++;
+            }
+            if (i >= npre) {
+                mbar_wait(w_empty(i % W_SLOTS), (i / W_SLOTS - 1) & 1);
+                if (elect_one()) load_w(i);
+                __syncwarp();
+            }
+            if (i == 0 && lane == 0 && tr_first) tr_first[2] = clock64();
+        }
+        if (lane == 0 && tr_first) tr_first[3] = clock64();
+    } else {
+        // ===================== consumer warpgroups =====================
+        const int wg = warp >> 2;
+        const uint32_t a_off = (uint32_t)wg * 8192u;     // the warpgroup's 64 rows of the A tile
+        pdl_wait();      // bias / residual reads and the stores below touch buffers of earlier kernels
+        const bool splitk = gridDim.z > 1, lead = blockIdx.z == 0;
+        int i = 0, ag = 0;     // W k-blocks consumed; A k-blocks of the tiles before the current A group
+        for (int rr = 0; rr < nrows; rr++) {
+            const int r = blockIdx.y + rr * gridDim.y, m0 = r * BM;
+            for (int cc = 0; cc < ncols; cc++) {
+                const int c = c_begin + cc, n0 = c * BN;
+                long long* const tr = rec(r, c);
+                if (threadIdx.x == 0 && tr && (rr || cc)) tr[0] = clock64();
+                const bool last_use = !resident || cc == ncols - 1;      // of the A k-blocks
+                if (zero_ptr) {
+                    // side job: clear this tile's patch of an auxiliary matrix (the zeroed C that the NEXT split-K GEMM reduces into)
+                    const int zc4 = zero_cols / ct / 4;
+                    for (int j = threadIdx.x; j < BM * zc4; j += GEMM_CW * 32) {
+                        const int rz = j / zc4, c4 = j % zc4;
+                        if (m0 + rz < M)
+                            *reinterpret_cast<float4*>(zero_ptr + (size_t)(m0 + rz) * zero_ld + (c * zc4 + c4) * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
+                    }
+                }
+                float sum[NR], part[NR], small[NR];
+#pragma unroll
+                for (int j = 0; j < NR; j++) sum[j] = 0.f;
+                for (int kb = 0; kb < num_kb; kb++, i++) {
+                    const int sa = (ag + kb) % A_SLOTS, sw = i % W_SLOTS;
+                    mbar_wait(a_full(sa), ((ag + kb) / A_SLOTS) & 1);
+                    mbar_wait(w_full(sw), (i / W_SLOTS) & 1);
+                    if (kb == 0 && threadIdx.x == 0 && tr) tr[6] = clock64();
+                    const uint32_t a_hi = base + sa * A_BYTES + a_off, w_hi = base + W_OFF + sw * W_BYTES;
+                    wgmma_fence();
+                    // debug bit 64: hi x hi only (MMA throughput probe)
+                    split_kblock(part, small, make_smem_desc(a_hi), make_smem_desc(a_hi + A_BYTES / 2), make_smem_desc(w_hi),
+                                 make_smem_desc(w_hi + W_BYTES / 2), kb % promote == 0, kb == 0, !(epi & 64));
+                    wgmma_commit();
+                    wgmma_wait0();
+                    __syncwarp();
+                    if (lane == 0) {       // slots reusable once this warp's MMAs have read them
+                        mbar_arrive(w_empty(sw));
+                        if (last_use) mbar_arrive(a_empty(sa));
+                    }
+                    if ((kb + 1) % promote == 0 || kb == num_kb - 1) {
+#pragma unroll
+                        for (int j = 0; j < NR; j++) sum[j] += part[j];
+                    }
+                }
+                if (last_use) ag += num_kb;
+                if (threadIdx.x == 0 && tr) tr[9] = clock64();
+                // ---- epilogue.  The warp's 16 rows of sum + 2^-11 small go through shared memory (accumulator layout in: rows
+                // lane / 4 (+ 8), columns 8 j + 2 (lane % 4); XOR swizzle of the column by 8 (row % 4) keeps the float2 writes of a
+                // half-warp on distinct banks), then out row by row, 16 lanes x float4 per row: every store instruction writes two
+                // whole 256-byte row segments instead of 8-byte pieces of 8 rows.  Then bias / GELU / SiLU, residual, stores.
+                float* const stage = reinterpret_cast<float*>(smem_raw + (base - smem_u32(smem_raw)) + E_OFF + warp * E_BYTES);
+                {
+                    const int rl = lane >> 2, cq = 2 * (lane & 3);
+#pragma unroll
+                    for (int j = 0; j < BN / 8; j++) {
+#pragma unroll
+                        for (int hh = 0; hh < 2; hh++) {
+                            const int row = rl + 8 * hh, e = 4 * j + 2 * hh;
+                            const float2 v = (epi & 64) ? make_float2(sum[e], sum[e + 1])
+                                                        : make_float2(fmaf(small[e], 1.0f / 2048.0f, sum[e]), fmaf(small[e + 1], 1.0f / 2048.0f, sum[e + 1]));
+                            *reinterpret_cast<float2*>(stage + row * BN + ((8 * j + cq) ^ (8 * (row & 3)))) = v;
+                        }
+                    }
+                }
+                __syncwarp();
+                {
+                    const int cl = 4 * (lane & 15), col = n0 + cl;      // N is a multiple of 4: col < N implies col + 3 < N
+                    float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
+                    if ((epi & EPI_BIAS) && lead && col < N) b4 = *reinterpret_cast<const float4*>(bias + col);
+#pragma unroll 2
+                    for (int it = 0; it < 8; it++) {
+                        const int rl = 2 * it + (lane >> 4), row = m0 + wg * 64 + (warp & 3) * 16 + rl;
+                        if (row >= M || col >= N) continue;
+                        float4 o = *reinterpret_cast<const float4*>(stage + rl * BN + (cl ^ (8 * (rl & 3))));
+                        o.x += b4.x; o.y += b4.y; o.z += b4.z; o.w += b4.w;
+                        if (epi & EPI_GELU) { o.x = gelu_erf(o.x); o.y = gelu_erf(o.y); o.z = gelu_erf(o.z); o.w = gelu_erf(o.w); }
+                        if (epi & EPI_SILU) { o.x = silu(o.x); o.y = silu(o.y); o.z = silu(o.z); o.w = silu(o.w); }
+                        if ((epi & EPI_RES) && lead) {
+                            const float4 r4 = *reinterpret_cast<const float4*>(res + (size_t)row * ldr + col);
+                            o.x += r4.x; o.y += r4.y; o.z += r4.z; o.w += r4.w;
+                        }
+                        if (splitk) {
+                            asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(C + (size_t)row * ldc + col), "f"(o.x), "f"(o.y),
+                                         "f"(o.z), "f"(o.w) : "memory");
+                        } else if (C) *reinterpret_cast<float4*>(C + (size_t)row * ldc + col) = o;
+                        if (Ch) {
+                            __half2 h01, l01, h23, l23;
+                            split_f16x2(o.x, o.y, h01, l01);
+                            split_f16x2(o.z, o.w, h23, l23);
+                            *reinterpret_cast<uint2*>(Ch + (size_t)row * ldc + col) = make_uint2(*reinterpret_cast<uint32_t*>(&h01), *reinterpret_cast<uint32_t*>(&h23));
+                            *reinterpret_cast<uint2*>(Cl + (size_t)row * ldc + col) = make_uint2(*reinterpret_cast<uint32_t*>(&l01), *reinterpret_cast<uint32_t*>(&l23));
+                        }
+                    }
+                }
+                __syncwarp();      // the staging rows are rewritten by the next tile
+                if (threadIdx.x == 0 && tr) tr[10] = clock64();
+            }
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        long long* const tr = rec(blockIdx.y + (nrows - 1) * gridDim.y, c_begin + ncols - 1);
+        if (tr) { tr[11] = clock64(); if (tr != tr_first) tr[12] = t_entry; }
+        chain_mark(1, 2);
+    }
+}
+
 // stand-alone launch of the feed-forward block: grid (8, ceil(M / 128)), one 128-row tile per cluster
 __global__ void __cluster_dims__(mlp::CLUSTER, 1, 1) __launch_bounds__(NUM_THREADS, 1)
 mlp_fused_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w1,
@@ -269,6 +490,7 @@ CHAIN_SETTER(idb_chain_set_gemm)
 long long* g_idb_gemm_trace = nullptr;   // set by the debug hooks for ONE following launch
 int g_idb_gemm_wide_tiles = 1;           // 128-column tiles where idb_gemm_wgmma picks them; 0 = 64-column tiles everywhere (test hook)
 int g_idb_gemm_promote = 0;              // 0 = default; test hook (idb_debug_set_gemm_accumulators)
+int g_idb_gemm_persistent = 1;           // 0 = one tile per CTA in the 64-column kernel (test hook)
 
 bool idb_gemm_wgmma_supported(const GemmArgs& g) {
     // TMA needs 16-byte aligned row strides (8 fp16); the vector epilogue needs ldc % 4 == 0
@@ -287,7 +509,7 @@ int idb_gemm_wgmma(idb_handle* h, const GemmArgs& g, cudaStream_t st) {
     if ((g.epi & EPI_BIAS) && mis(g.bias)) return idb_fail(h, IDB_ERR_ARG, "bias must be 16-byte aligned");
     if (!(h->attr_mask & 1u)) {      // per handle = per device (function attributes live in the device's context)
         CUDA_TRY(h, cudaFuncSetAttribute(gemm_split_f16_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<128>::SMEM_BYTES));
-        CUDA_TRY(h, cudaFuncSetAttribute(gemm_split_f16_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<64>::SMEM_BYTES));
+        CUDA_TRY(h, cudaFuncSetAttribute(gemm_split_f16_persistent, cudaFuncAttributeMaxDynamicSharedMemorySize, pers::SMEM_BYTES));
         CUDA_TRY(h, cudaFuncSetAttribute(gemm_split_f16_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<128>::SMEM_BYTES));
         h->attr_mask |= 1u;
     }
@@ -340,9 +562,16 @@ int idb_gemm_wgmma(idb_handle* h, const GemmArgs& g, cudaStream_t st) {
     } else {
         if ((rc = make_map(h, &mw, g.W_hi, N, K, g.ldw, 64))) return rc;
         if ((rc = make_map(h, &mwl, g.W_lo, N, K, g.ldw, 64))) return rc;
-        dim3 grid((N + 63) / 64, row_tiles, ksplit);
-        idb_launch(g.pdl != 0, gemm_split_f16_kernel<64>, grid, GEMM_THREADS, Cfg<64>::SMEM_BYTES, st, ma, mw, mal, mwl, g.bias, g.res, g.ldr,
-                   g.C, g.C_hi, g.C_lo, g.ldc, M, N, K, g.epi, promote, zero, g.zero_ld, g.zero_cols, trace);
+        // at most one CTA per SM: the CTAs of a row tile split its column tiles, and a grid short of rows takes further row
+        // tiles in turn (gemm_split_f16_persistent)
+        const int col_tiles = (N + 63) / 64, sms = std::max(1, h->sm_count / ksplit);
+        int cpr = col_tiles, gy = row_tiles;
+        if (g_idb_gemm_persistent) {
+            gy = std::min(row_tiles, sms);
+            cpr = std::max(1, std::min(col_tiles, sms / row_tiles));
+        }
+        idb_launch(g.pdl != 0, gemm_split_f16_persistent, dim3(cpr, gy, ksplit), GEMM_THREADS, pers::SMEM_BYTES, st, ma, mw, mal, mwl, g.bias,
+                   g.res, g.ldr, g.C, g.C_hi, g.C_lo, g.ldc, M, N, K, g.epi, promote, zero, g.zero_ld, g.zero_cols, trace);
     }
     LAUNCH_CHECK(h);
     return IDB_OK;
