@@ -266,6 +266,33 @@ int idb_debug_attn_trace(long long* out16);
    kernel of the sampling step then appends (kind | event | grid | block, %globaltimer) records; NULL switches it off */
 int idb_debug_chain_trace(idb_handle* h, unsigned long long* buf);
 
+/* One launch of a per-sample attention kernel of the denoiser on caller operands (fp32 device pointers, rows m = b*T + t,
+ * row stride 256 unless given), with the grid, block, shared memory and launch attribute the decoder / encoder use.
+ * kernel: 0 self-attention + LN1 (k_attn_ln), 1 cross-attention + LN2 (k_xattn_ln), 2 both in one launch (k_attn_xattn_ln;
+ * x1_out receives the LN1 rows), 3 QaN + LN1 + cross-attention + LN2 with a pending LayerNorm `pre` on the input rows
+ * (k_qan_xattn_ln<true, true>), 4 the same without one (k_qan_xattn_ln<true, false>), 5 QaN + LN1 of an encoder layer
+ * (k_qan_xattn_ln<false>; `pre` optional).
+ *   self:  q, k (head h at columns 64h.., row strides ldq / ldk), v (out-projection folded in: head h at columns 256h.., ldv),
+ *          res, bo, ln1:  out = LN1(res + bo + sum_h sum_j softmax_j(q_h . k_h / 8) v_h[j])
+ *   cross: x1 (kernel 1; else the LN1 rows), memory kp, vp [Tk*B][H*256], kc [Tk*B][H] (rows j*B + b), bo2, ln2:
+ *          out = LN2(x1 + bo2 + sum_{h,j} softmax_j(x1 . kp_h[j] + kc_h[j]) vp_h[j])
+ *   QaN:   zin, pre, qt [3][N][256] (folded queries, packed as idb_denoiser_commit packs them), wk [N], ln1
+ * out_hi / out_lo (optional): the output's fp16 (hi, lo) pairs too.  H must be 4, T <= 36, Tk <= 16 (>= 1 with a
+ * cross-attention block), N <= 10; anything else is IDB_ERR_ARG.  Rows >= B*T of the outputs are not written. */
+typedef struct {
+    int kernel, B, T, Tk, N, H, pdl;
+    const float* q; int ldq; const float* k; int ldk; const float* v; int ldv;
+    const float* res; const float* bo; const float* ln1_w; const float* ln1_b;
+    const float* x1; const float* kp; const float* vp; const float* kc; const float* bo2; const float* ln2_w; const float* ln2_b;
+    const float* zin; const float* pre_w; const float* pre_b; const float* qt; const float* wk;
+    float* out; void* out_hi; void* out_lo; float* x1_out;
+} idb_attn_desc;
+int idb_debug_attention(idb_handle* h, const idb_attn_desc* d, void* stream);
+/* copies one fp32 tensor of decoder layer `layer` as committed (bound, for the memory tensors) to dst (count elements, exactly
+ * the tensor's size): "qkvf_w" [(2 + H) 256][256], "qkvf_b" [(2 + H) 256], "bo_f" [256] (standard layers), "qt" [3N][256] (QaN
+ * layers), "kp", "vp" [Tk*B][H*256], "kc" [Tk*B][H].  A tensor the layer does not have, or a wrong count, is IDB_ERR_ARG. */
+int idb_debug_denoiser_tensor(idb_handle* h, int layer, const char* name, float* dst, long long count);
+
 /* debug: fp16 (hi, lo) operand split (x = hi + lo * 2^-11), and a GEMM on such pairs */
 int idb_debug_split(idb_handle* h, const float* x, void* hi, void* lo, int rows, int cols, int ld_dst, void* stream);
 int idb_debug_gemm_presplit(idb_handle* h, const void* A_hi, const void* A_lo, const void* W_hi, const void* W_lo,

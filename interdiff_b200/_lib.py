@@ -29,6 +29,17 @@ class GemmDesc(C.Structure):
                 ("trace", C.c_void_p)]
 
 
+class AttnDesc(C.Structure):
+    """idb_attn_desc: one per-sample attention kernel launch on caller operands (idb_debug_attention)."""
+    _fields_ = [("kernel", C.c_int), ("B", C.c_int), ("T", C.c_int), ("Tk", C.c_int), ("N", C.c_int), ("H", C.c_int), ("pdl", C.c_int),
+                ("q", C.c_void_p), ("ldq", C.c_int), ("k", C.c_void_p), ("ldk", C.c_int), ("v", C.c_void_p), ("ldv", C.c_int),
+                ("res", C.c_void_p), ("bo", C.c_void_p), ("ln1_w", C.c_void_p), ("ln1_b", C.c_void_p),
+                ("x1", C.c_void_p), ("kp", C.c_void_p), ("vp", C.c_void_p), ("kc", C.c_void_p), ("bo2", C.c_void_p),
+                ("ln2_w", C.c_void_p), ("ln2_b", C.c_void_p),
+                ("zin", C.c_void_p), ("pre_w", C.c_void_p), ("pre_b", C.c_void_p), ("qt", C.c_void_p), ("wk", C.c_void_p),
+                ("out", C.c_void_p), ("out_hi", C.c_void_p), ("out_lo", C.c_void_p), ("x1_out", C.c_void_p)]
+
+
 _P = C.c_void_p
 _SIGS = {
     "idb_version": (C.c_int, []),
@@ -80,6 +91,8 @@ _SIGS = {
     "idb_debug_split": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P]),
     "idb_debug_gemm_presplit": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "idb_debug_chain_trace": (C.c_int, [_P, _P]),
+    "idb_debug_attention": (C.c_int, [_P, C.POINTER(AttnDesc), _P]),
+    "idb_debug_denoiser_tensor": (C.c_int, [_P, C.c_int, C.c_char_p, _P, C.c_longlong]),
     "idb_correction_apply": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, _P, _P]),
     "idb_projector_init_skeleton": (C.c_int, [_P, C.c_int, C.c_int, C.c_int]),
     "idb_projector_sample_skeleton": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P]),

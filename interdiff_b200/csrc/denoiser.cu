@@ -1190,6 +1190,19 @@ struct Packer {
 };
 }  // namespace
 
+// folded queries as fp16 (hi, lo), rows padded to the stride the kernels keep in shared memory: one block
+// [2 (hi, lo)][3N][KPH] (pad columns zero).  qb / qs: the [3N][D] split of qt, written on the legacy default stream.
+static size_t qt_pack_bytes(int N) { return 2 * (size_t)3 * N * KPH * sizeof(__half); }
+static int pack_queries(idb_handle* h, const __half* qb, const __half* qs, int N, __half* pack) {
+    CUDA_TRY(h, cudaDeviceSynchronize());      // the split kernels ran on the handle's stream
+    const size_t half_bytes = qt_pack_bytes(N) / 2;
+    CUDA_TRY(h, cudaMemset(pack, 0, 2 * half_bytes));
+    CUDA_TRY(h, cudaMemcpy2D(pack, KPH * sizeof(__half), qb, D * sizeof(__half), D * sizeof(__half), 3 * N, cudaMemcpyDeviceToDevice));
+    CUDA_TRY(h, cudaMemcpy2D(reinterpret_cast<uint8_t*>(pack) + half_bytes, KPH * sizeof(__half), qs, D * sizeof(__half),
+                             D * sizeof(__half), 3 * N, cudaMemcpyDeviceToDevice));
+    return IDB_OK;
+}
+
 extern "C" int idb_denoiser_commit(idb_handle* h) {
     IDB_ENTER(h);
     if (!h) return IDB_ERR_ARG;
@@ -1379,18 +1392,12 @@ extern "C" int idb_denoiser_commit(idb_handle* h) {
             for (auto& L : *stack) {
                 if (!rc && !L.qan) rc = split(L.w_qkvf, 2 * D + H * D, D, D, &L.w_qkvf_b, &L.w_qkvf_s);
                 if (!rc && L.qan) {
-                    // folded queries as fp16 (hi, lo), rows padded to the stride the kernels keep in shared memory: one block
                     __half *qb = nullptr, *qs = nullptr;
                     rc = split(L.qt, 3 * N, D, D, &qb, &qs);
                     if (!rc) {
-                        CUDA_TRY(h, cudaDeviceSynchronize());      // the split kernels ran on the handle's stream
-                        const size_t half_bytes = (size_t)3 * N * KPH * sizeof(__half);
-                        CUDA_TRY(h, cudaMalloc((void**)&L.qt_pack, 2 * half_bytes));
+                        CUDA_TRY(h, cudaMalloc((void**)&L.qt_pack, qt_pack_bytes(N)));
                         d.owned.push_back(reinterpret_cast<float*>(L.qt_pack));
-                        CUDA_TRY(h, cudaMemset(L.qt_pack, 0, 2 * half_bytes));
-                        CUDA_TRY(h, cudaMemcpy2D(L.qt_pack, KPH * sizeof(__half), qb, D * sizeof(__half), D * sizeof(__half), 3 * N, cudaMemcpyDeviceToDevice));
-                        CUDA_TRY(h, cudaMemcpy2D(reinterpret_cast<uint8_t*>(L.qt_pack) + half_bytes, KPH * sizeof(__half), qs, D * sizeof(__half),
-                                                 D * sizeof(__half), 3 * N, cudaMemcpyDeviceToDevice));
+                        rc = pack_queries(h, qb, qs, N, L.qt_pack);
                     }
                 }
                 if (!rc) rc = split(L.w1, F, D, D, &L.w1_b, &L.w1_s);
@@ -1678,6 +1685,118 @@ int idb_denoiser_prepare_kernels(idb_handle* h) {
     CUDA_TRY(h, cudaFuncSetAttribute(k_attn_ln, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_smem(36, 4)));
     CUDA_TRY(h, cudaFuncSetAttribute(k_attn_xattn_ln, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (int)(attn_smem(36, 4) > xattn_smem(16, 4) ? attn_smem(36, 4) : xattn_smem(16, 4))));
+    return IDB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Test hooks: one attention kernel on caller operands, and read-back of a layer's folded operands.
+extern "C" int idb_debug_attention(idb_handle* h, const idb_attn_desc* a, void* stream) {
+    IDB_ENTER(h);
+    if (!h || !a) return IDB_ERR_ARG;
+    const int kind = a->kernel, B = a->B, T = a->T, Tk = a->Tk, N = a->N, H = a->H;
+    const bool self = kind == 0 || kind == 2, qan = kind >= 3, cross = kind >= 1 && kind <= 4;
+    if (kind < 0 || kind > 5) return idb_fail(h, IDB_ERR_ARG, "idb_debug_attention: kernel must be 0 .. 5");
+    if (H != 4 || B < 1 || T < 1 || T > 36 || Tk < 0 || Tk > 16 || (cross && Tk < 1) || (qan && (N < 1 || N > 10)))
+        return idb_fail(h, IDB_ERR_ARG, "idb_debug_attention: supported H = 4, 1 <= T <= 36, Tk <= 16 (>= 1 with cross-attention), 1 <= N <= 10");
+    if (!a->out || (!a->out_hi) != (!a->out_lo) || (kind != 1 && (!a->ln1_w || !a->ln1_b)) || (kind == 1 && !a->x1) || (kind == 2 && !a->x1_out) ||
+        (self && (!a->q || !a->k || !a->v || !a->res || !a->bo)) || (cross && (!a->kp || !a->vp || !a->kc || !a->bo2 || !a->ln2_w || !a->ln2_b)) ||
+        (qan && (!a->zin || !a->qt || !a->wk)) || (kind == 3 && !a->pre_w) || (kind == 4 && a->pre_w) || (!a->pre_w) != (!a->pre_b))
+        return idb_fail(h, IDB_ERR_ARG, "idb_debug_attention: missing operand");
+    cudaStream_t st = (cudaStream_t)stream;
+    const dim3 grid(B, (T + SLAB - 1) / SLAB);
+    const bool pdl = a->pdl != 0;
+    __half* out_b = (__half*)a->out_hi; __half* out_s = (__half*)a->out_lo;
+    std::vector<void*> tmp;
+    auto release = [&]() { for (void* p : tmp) cudaFree(p); };      // cudaFree waits for the device
+    auto alloc = [&](size_t bytes) -> void* {
+        void* p = nullptr;
+        if (cudaMalloc(&p, bytes) != cudaSuccess) return nullptr;
+        tmp.push_back(p);
+        return p;
+    };
+    int rc = IDB_OK;
+    uint8_t* mpack = nullptr;
+    if (cross) {     // the memory tensors packed as idb_denoiser_bind packs them
+        const size_t bytes = (size_t)B * mem_block_bytes(H * Tk);
+        mpack = (uint8_t*)alloc(bytes);
+        if (!mpack) { release(); return idb_fail(h, IDB_ERR_CUDA, "idb_debug_attention: out of device memory"); }
+        cudaMemsetAsync(mpack, 0, bytes, st);
+        k_pack_memory<<<dim3(H * Tk, B), D, 0, st>>>(a->kp, a->vp, a->kc, mpack, B, Tk, H);
+        h->launches++;
+        if (cudaGetLastError() != cudaSuccess) { release(); return idb_fail(h, IDB_ERR_CUDA, "k_pack_memory launch failed"); }
+    }
+    __half* qpack = nullptr;
+    if (qan) {       // the folded queries packed as idb_denoiser_commit packs them
+        __half* qb = (__half*)alloc((size_t)3 * N * D * sizeof(__half));
+        __half* qs = (__half*)alloc((size_t)3 * N * D * sizeof(__half));
+        qpack = (__half*)alloc(qt_pack_bytes(N));
+        if (!qb || !qs || !qpack) { release(); return idb_fail(h, IDB_ERR_CUDA, "idb_debug_attention: out of device memory"); }
+        const cudaError_t e = cudaStreamSynchronize(st);          // qt may have been written on the caller's stream
+        if (e != cudaSuccess) { release(); return idb_fail(h, IDB_ERR_CUDA, "idb_debug_attention: %s", cudaGetErrorString(e)); }
+        rc = idb_split_tensor(h, a->qt, D, qb, qs, D, 3 * N, D, 0);
+        if (!rc) rc = pack_queries(h, qb, qs, N, qpack);
+        if (rc) { release(); return rc; }
+    }
+    AttnArgs aa = {};
+    aa.q = a->q; aa.ldq = a->ldq ? a->ldq : D; aa.k = a->k; aa.ldk = a->ldk ? a->ldk : D; aa.v = a->v; aa.ldv = a->ldv ? a->ldv : H * D;
+    aa.res = a->res; aa.bo = a->bo; aa.lnw = a->ln1_w; aa.lnb = a->ln1_b; aa.T = T; aa.H = H;
+    XattnArgs xa = {};
+    xa.mpack = mpack; xa.bo = a->bo2; xa.lnw = a->ln2_w; xa.lnb = a->ln2_b; xa.out = a->out; xa.out_b = out_b; xa.out_s = out_s;
+    xa.T = T; xa.B = B; xa.Tk = Tk; xa.H = H;
+    QanArgs qa = {};
+    qa.zin = a->zin; qa.prew = a->pre_w; qa.preb = a->pre_b; qa.qpack = qpack; qa.wk = a->wk; qa.lnw = a->ln1_w; qa.lnb = a->ln1_b;
+    qa.mpack = mpack; qa.bo2 = a->bo2; qa.ln2w = a->ln2_w; qa.ln2b = a->ln2_b; qa.out = a->out; qa.out_b = out_b; qa.out_s = out_s;
+    qa.T = T; qa.N = N; qa.B = B; qa.Tk = Tk; qa.H = H;
+    cudaError_t e = cudaSuccess;
+    switch (kind) {
+        case 0:
+            aa.out = a->out; aa.out_b = out_b; aa.out_s = out_s;
+            e = idb_launch(pdl, k_attn_ln, grid, ANT, attn_smem(T, H), st, aa);
+            break;
+        case 1:
+            xa.x1 = a->x1;
+            e = idb_launch(pdl, k_xattn_ln, grid, ANT, xattn_smem(Tk, H), st, xa);
+            break;
+        case 2: {
+            aa.out = a->x1_out; xa.x1 = a->x1_out;
+            const size_t smem = attn_smem(T, H) > xattn_smem(Tk, H) ? attn_smem(T, H) : xattn_smem(Tk, H);
+            e = idb_launch(pdl, k_attn_xattn_ln, grid, ANT, smem, st, aa, xa);
+            break;
+        }
+        case 3: e = idb_launch(pdl, k_qan_xattn_ln<true, true>, grid, ANT, qan_smem(Tk, H), st, qa); break;
+        case 4: e = idb_launch(pdl, k_qan_xattn_ln<true, false>, grid, ANT, qan_smem(Tk, H), st, qa); break;
+        default: e = idb_launch(pdl, k_qan_xattn_ln<false>, grid, ANT, qan_enc_smem(), st, qa); break;
+    }
+    h->launches++;
+    if (e == cudaSuccess) e = cudaGetLastError();
+    release();
+    if (e != cudaSuccess) return idb_fail(h, IDB_ERR_CUDA, "idb_debug_attention: %s", cudaGetErrorString(e));
+    return IDB_OK;
+}
+
+extern "C" int idb_debug_denoiser_tensor(idb_handle* h, int layer, const char* name, float* dst, long long count) {
+    IDB_ENTER(h);
+    if (!h || !name || !dst) return IDB_ERR_ARG;
+    Denoiser& d = h->den;
+    if (!d.committed) return idb_fail(h, IDB_ERR_STATE, "idb_denoiser_commit first");
+    if (layer < 0 || layer >= (int)d.layers.size()) return idb_fail(h, IDB_ERR_ARG, "no decoder layer %d", layer);
+    const DenoiserLayer& L = d.layers[layer];
+    const int H = d.cfg.n_heads, N = d.cfg.n_queries;
+    const size_t mem_rows = (size_t)d.Tm * d.B;
+    const std::string s(name);
+    const float* src = nullptr;
+    size_t n = 0;
+    if (s == "qkvf_w") { src = L.w_qkvf; n = (size_t)(2 * D + H * D) * D; }
+    else if (s == "qkvf_b") { src = L.b_qkvf; n = (size_t)2 * D + H * D; }
+    else if (s == "bo_f") { src = L.bo_f; n = D; }
+    else if (s == "qt") { src = L.qt; n = (size_t)3 * N * D; }
+    else if (s == "kp") { src = d.B ? L.kp_mem : nullptr; n = mem_rows * H * D; }
+    else if (s == "vp") { src = d.B ? L.vp_mem : nullptr; n = mem_rows * H * D; }
+    else if (s == "kc") { src = d.B ? L.kc_mem : nullptr; n = mem_rows * H; }
+    if (!src) return idb_fail(h, IDB_ERR_ARG, "decoder layer %d has no tensor '%s' (committed%s)", layer, name, d.B ? " and bound" : ", not bound");
+    if ((size_t)count != n) return idb_fail(h, IDB_ERR_ARG, "tensor '%s' has %zu elements, not %lld", name, n, count);
+    CUDA_TRY(h, cudaDeviceSynchronize());
+    CUDA_TRY(h, cudaMemcpy(dst, src, n * sizeof(float), cudaMemcpyDefault));
     return IDB_OK;
 }
 

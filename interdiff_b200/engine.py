@@ -192,6 +192,54 @@ class Engine:
         self._chk(self.lib.idb_debug_gemm_ex(self._h, C.byref(d), self._stream()))
         return out if out is not None else out_pair
 
+    ATTN_KERNELS = {"attn_ln": 0, "xattn_ln": 1, "attn_xattn_ln": 2, "qan_xattn_ln_pre": 3, "qan_xattn_ln": 4, "qan_ln": 5}
+
+    def attention(self, kernel, B, T, Tk=0, N=0, *, q=None, k=None, v=None, res=None, bo=None, ln1=None, x1=None, kp=None,
+                  vp=None, kc=None, bo2=None, ln2=None, zin=None, pre=None, qt=None, wk=None, out=None, out_pair=None,
+                  x1_out=None, pdl=False, H=4):
+        """One per-sample attention kernel of the denoiser on these operands, via idb_debug_attention (tests).
+        kernel: "attn_ln" (self-attention + LN1), "xattn_ln" (cross-attention + LN2), "attn_xattn_ln" (both, one launch),
+        "qan_xattn_ln_pre" / "qan_xattn_ln" (QaN decoder layer with / without the pending norm `pre`), "qan_ln" (QaN encoder
+        layer, `pre` optional).  q, k, v: fp32 matrices, views of wider buffers keep their row stride; the norms ln1 / ln2 /
+        pre are (weight, bias) pairs; qt [3N][256]; the memory kp, vp [Tk*B][H*256], kc [Tk*B][H].  out: [>= B*T, 256] fp32
+        (rows past B*T are left as they are), out_pair: fp16 (hi, lo) tensors of out's shape, x1_out: the LN1 rows of
+        "attn_xattn_ln".  Returns out."""
+        f = lambda t: self._f32(t) if t is not None else None
+        rows = lambda t: self._rows(t, torch.float32) if t is not None else None
+        q, k, v = rows(q), rows(k), rows(v)
+        res, bo, x1, kp, vp, kc, bo2, zin, qt, wk = (f(t) for t in (res, bo, x1, kp, vp, kc, bo2, zin, qt, wk))
+        ln1, ln2, pre = ((f(p[0]), f(p[1])) if p is not None else (None, None) for p in (ln1, ln2, pre))
+        if out is None:
+            out = torch.empty(B * T, 256, device=self.device)
+        for t, dt in [(out, torch.float32), (x1_out, torch.float32)] + [(t, torch.float16) for t in (out_pair or ())]:
+            if t is not None and not (t.device == self.device and t.dtype == dt and t.is_contiguous() and t.dim() == 2
+                                      and t.shape[1] == 256 and t.shape[0] >= B * T):
+                raise EngineError("attention: outputs are contiguous [>= B*T, 256] device tensors")
+        d = _lib.AttnDesc()
+        d.kernel, d.B, d.T, d.Tk, d.N, d.H, d.pdl = self.ATTN_KERNELS[kernel], B, T, Tk, N, H, int(bool(pdl))
+        P = self._ptr
+        d.q, d.k, d.v = P(q), P(k), P(v)
+        d.ldq, d.ldk, d.ldv = (t.stride(0) if t is not None else 0 for t in (q, k, v))
+        d.res, d.bo, d.ln1_w, d.ln1_b = P(res), P(bo), P(ln1[0]), P(ln1[1])
+        d.x1, d.kp, d.vp, d.kc, d.bo2, d.ln2_w, d.ln2_b = P(x1), P(kp), P(vp), P(kc), P(bo2), P(ln2[0]), P(ln2[1])
+        d.zin, d.pre_w, d.pre_b, d.qt, d.wk = P(zin), P(pre[0]), P(pre[1]), P(qt), P(wk)
+        d.out, d.x1_out = P(out), P(x1_out)
+        if out_pair is not None:
+            d.out_hi, d.out_lo = P(out_pair[0]), P(out_pair[1])
+        self._chk(self.lib.idb_debug_attention(self._h, C.byref(d), self._stream()))
+        return out
+
+    def denoiser_tensor(self, layer, name):
+        """A folded operand of decoder layer `layer` as the library committed / bound it (idb_debug_denoiser_tensor):
+        qkvf_w, qkvf_b, bo_f (standard layers), qt (QaN layers), kp, vp, kc (after bind); fp32 device tensor."""
+        H, N, D = self.n_heads, self.n_queries, self.D
+        mem = getattr(self, "Tm", 0) * getattr(self, "B", 0)
+        shape = {"qkvf_w": ((2 + H) * D, D), "qkvf_b": ((2 + H) * D,), "bo_f": (D,), "qt": (3 * N, D),
+                 "kp": (mem, H * D), "vp": (mem, H * D), "kc": (mem, H)}[name]
+        out = torch.empty(shape, device=self.device)
+        self._chk(self.lib.idb_debug_denoiser_tensor(self._h, int(layer), name.encode(), self._ptr(out), out.numel()))
+        return out
+
     def gemm_microbench(self, M, N, K, iters=200, gelu=True, split_k=False):
         """Mean device time of one tensor-core GEMM launch (fp16-pair operands as the denoiser feeds them,
         bias + optional GELU epilogue) over `iters` back-to-back launches issued from C on the current
@@ -250,7 +298,7 @@ class Engine:
         self._chk(self.lib.idb_denoiser_commit(self._h))
         self.variant = variant
         self.C = cfg.c_body + cfg.c_obj + cfg.c_extra
-        self.D = D
+        self.D, self.n_heads, self.n_queries = D, n_heads, n_queries
 
     def bind(self, cond, T, zero_pose_obj=None):
         """cond (Tm,B,D) as in model_kwargs['y']['cond']."""
@@ -259,7 +307,7 @@ class Engine:
         zp = self._f32(zero_pose_obj) if zero_pose_obj is not None else None
         self._chk(self.lib.idb_denoiser_bind(self._h, B, T, Tm, self._ptr(cond), self._ptr(zp), self._stream()))
         self._keep = [cond, zp]
-        self.B, self.T = B, T
+        self.B, self.T, self.Tm = B, T, Tm
 
     def forward(self, x, timesteps):
         x = self._f32(x)
