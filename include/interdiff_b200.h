@@ -86,6 +86,17 @@ int idb_denoiser_forward(idb_handle* h, const float* x, const int64_t* timesteps
  *   cond_out     (Tp,B,256)  sequence-first like the reference; feed it to idb_denoiser_bind */
 int idb_encode_condition(idb_handle* h, int B, int Tp, const float* past, const float* pc_embedding, float* cond_out, void* stream);
 
+/* Conditioning encoder of the skeleton model = MDM._get_embeddings (reference model/diffusion_skeleton.py:194-215):
+ *   cond = encoder(PositionalEmbedding(bodyEmbedding(body[:Tp]) + objEmbedding(obj[:Tp]) + shapeEmbedding(zero_pose_obj)))
+ * Needs the "encoder.layers.*" and "shapeEmbedding.*" tensors loaded before idb_denoiser_commit; skeleton variant only.
+ *   body          (>=Tp,B,n_joints,3)  sequence-first joints; only the first Tp frames are read
+ *   obj           (>=Tp,B,n_points,3)  sequence-first object keypoints; likewise
+ *   zero_pose_obj (B,n_points,3)       object keypoints in the canonical pose
+ *   cond_out      (Tp,B,256)           sequence-first; feed it to idb_denoiser_bind
+ * 1 <= Tp <= 36 (the encoder's attention window). */
+int idb_encode_condition_skeleton(idb_handle* h, int B, int Tp, const float* body, const float* obj, const float* zero_pose_obj,
+                                  float* cond_out, void* stream);
+
 /* PointNet++ (MSG) point-cloud encoder = MDM.pcEmbedding, PointNet2Encoder(c_in=1, c_out=256, num_keypoints=1)
  * (reference model/layers.py:111-175, called at model/diffusion_smpl.py:210-211); the furthest-point-sampling /
  * ball-query / grouping operators of the un-vendored pointnet2_ops 3.0.0 are rebuilt for sm_90a.

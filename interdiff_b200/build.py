@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libinterdiff_b200.so")
-SOURCES = ["api.cu", "gemm.cu", "gemm_wgmma.cu", "denoiser.cu", "sampler.cu", "lbs.cu", "geometry.cu", "correction.cu", "pointnet.cu", "metrics.cu", "rollout.cu"]
+SOURCES = ["api.cu", "gemm.cu", "gemm_wgmma.cu", "denoiser.cu", "sampler.cu", "lbs.cu", "geometry.cu", "correction.cu", "pointnet.cu", "metrics.cu", "rollout.cu", "skeleton_condition.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 

@@ -67,6 +67,7 @@ struct Denoiser {
     __half *e_xtok_b = nullptr, *e_xtok_s = nullptr, *e_h_b = nullptr, *e_h_s = nullptr, *e_h2_b = nullptr, *e_h2_s = nullptr,
            *e_ff_b = nullptr, *e_ff_s = nullptr;
     std::vector<void*> enc_owned;
+    const float *shp_w = nullptr, *shp_b = nullptr;   // skeleton shapeEmbedding [D][3 n_points], [D] (raw device copies)
     // PointNet++ point-cloud encoder (pointnet.cu): folded weights + workspace; optional like the encoder
     bool pn_ready = false; int pn_cap = 0;
     float *pn_w1 = nullptr, *pn_w2 = nullptr, *pn_xyz1 = nullptr, *pn_feat1 = nullptr;
@@ -277,6 +278,11 @@ struct GemmArgs {
 int idb_gemm_ex(idb_handle* h, const GemmArgs& g, cudaStream_t st);
 // fused feed-forward block on the tensor path (gemm_wgmma.cu)
 bool idb_mlp_wgmma_supported(int d_model, int d_ff);
+// token stage of the skeleton model's conditioning encoder (skeleton_condition.cu); widest shapeEmbedding input it takes
+constexpr int IDB_SHAPE_EMB_MAX_IN = 64;
+void idb_cond_tokens_skeleton(const float* body, const float* obj, const float* zero_pose_obj, const float* w_shape, const float* b_shape,
+                              const float* b_in, const float* pe, __half* xtok_b, __half* xtok_s, float* add, int B, int Tp, int Cb, int Co,
+                              int Cp, cudaStream_t st);
 int idb_mlp_wgmma(idb_handle* h, const __half* x_hi, const __half* x_lo, const __half* w1_hi, const __half* w1_lo, const float* b1,
                     const __half* w2_hi, const __half* w2_lo, const float* b2, const float* res, int ldr, float* Z, int ldz, int M,
                     int pdl, cudaStream_t st, const float* ln_w = nullptr, const float* ln_b = nullptr, __half* Z_hi = nullptr,

@@ -1120,6 +1120,7 @@ void idb_denoiser_release(idb_handle* h) {
     for (void* p : d.enc_owned) cudaFree(p);
     d.enc_owned.clear();
     d.enc_cap = 0;
+    d.shp_w = d.shp_b = nullptr;
     d.committed = false;
 }
 
@@ -1146,7 +1147,7 @@ extern "C" int idb_denoiser_load(idb_handle* h, const char* name, const float* d
     std::string s(name);
     // tensors of the sampling hot path and, when given, of the conditioning encoder (PointNet++ is a later row)
     bool want = s.rfind("decoder.layers.", 0) == 0 || s.rfind("encoder.layers.", 0) == 0 || s.rfind("pcEmbedding.", 0) == 0 ||
-                s.rfind("bodyEmbedding.", 0) == 0 || s.rfind("objEmbedding.", 0) == 0 ||
+                s.rfind("shapeEmbedding.", 0) == 0 || s.rfind("bodyEmbedding.", 0) == 0 || s.rfind("objEmbedding.", 0) == 0 ||
                 s.rfind("bodyFinalLinear.", 0) == 0 || s.rfind("objFinalLinear.", 0) == 0 ||
                 s.rfind("embedTimeStep.time_embed.", 0) == 0 || s == "PositionalEmbedding.pe";
     if (!want || s.find("inv_freq") != std::string::npos) return IDB_OK;
@@ -1370,6 +1371,12 @@ extern "C" int idb_denoiser_commit(idb_handle* h) {
             const int rc = build_layer("encoder.layers.", l, false, d.enc_layers);
             if (rc) return rc;
         }
+    }
+    // the skeleton encoder's object-shape embedding (optional like the encoder; model/diffusion_skeleton.py:19, :204)
+    d.shp_w = d.shp_b = nullptr;
+    if (c.variant == 1 && d.raw.count("shapeEmbedding.weight")) {
+        GET(w, "shapeEmbedding.weight", D, 3 * c.n_points) GET(b, "shapeEmbedding.bias", D)
+        d.shp_w = w->p; d.shp_b = b->p;
     }
 #undef GET
     if (P.rc) return P.rc;
@@ -1846,38 +1853,36 @@ __global__ void k_ln_seq_first(const float* __restrict__ a, const float* __restr
 
 }  // namespace
 
-extern "C" int idb_encode_condition(idb_handle* h, int B, int Tp, const float* past, const float* pc_embedding, float* cond_out,
-                                    void* stream) {
-    IDB_ENTER(h);
-    if (!h || !past || !pc_embedding || !cond_out || B <= 0 || Tp <= 0) return IDB_ERR_ARG;
+// Grows the encoder workspace to M token rows of Cp input channels.
+static int encoder_workspace(idb_handle* h, int M, int Cp) {
     Denoiser& d = h->den;
-    if (!d.committed) return idb_fail(h, IDB_ERR_STATE, "idb_denoiser_commit first");
-    if (d.enc_layers.empty()) return idb_fail(h, IDB_ERR_STATE, "the conditioning encoder's weights (encoder.layers.*) were not loaded");
-    if (Tp > 36) return idb_fail(h, IDB_ERR_ARG, "supported past window: <= 36 frames");
+    const int F = d.cfg.d_ff, H = d.cfg.n_heads;
+    if (M <= d.enc_cap) return IDB_OK;
+    for (void* p : d.enc_owned) cudaFree(p);
+    d.enc_owned.clear();
+    d.enc_cap = 0;
+    auto A = [&](float** p, size_t n) { if (cudaMalloc((void**)p, n * sizeof(float)) != cudaSuccess) return 1; d.enc_owned.push_back(*p); return 0; };
+    auto AH = [&](__half** p, size_t n) { if (cudaMalloc((void**)p, n * sizeof(__half)) != cudaSuccess) return 1; d.enc_owned.push_back(*p); return 0; };
+    int rc = 0;
+    rc |= A(&d.e_add, (size_t)M * D); rc |= A(&d.e_h, (size_t)M * D); rc |= A(&d.e_h2, (size_t)M * D); rc |= A(&d.e_z, (size_t)M * D);
+    rc |= A(&d.e_qkv, (size_t)M * (2 * D + H * D));
+    rc |= AH(&d.e_xtok_b, (size_t)M * Cp); rc |= AH(&d.e_xtok_s, (size_t)M * Cp);
+    rc |= AH(&d.e_h_b, (size_t)M * D); rc |= AH(&d.e_h_s, (size_t)M * D); rc |= AH(&d.e_h2_b, (size_t)M * D); rc |= AH(&d.e_h2_s, (size_t)M * D);
+    rc |= AH(&d.e_ff_b, (size_t)M * F); rc |= AH(&d.e_ff_s, (size_t)M * F);
+    if (rc) return idb_fail(h, IDB_ERR_CUDA, "out of device memory (encoder workspace)");
+    d.enc_cap = M;
+    return IDB_OK;
+}
+
+// Everything after the token stage, shared by both models: input GEMM (token pairs [B*Tp][Cp] @ W_in^T + addend), the
+// encoder layers, and the last norm into cond_out (Tp,B,D).
+static int encoder_layers(idb_handle* h, int B, int Tp, int Cp, float* cond_out, cudaStream_t st) {
+    Denoiser& d = h->den;
     const idb_denoiser_config& c = d.cfg;
-    const int M = B * Tp, F = c.d_ff, H = c.n_heads, N = c.n_queries, C = c.c_body + c.c_obj, Cp = (C + 7) & ~7;
-    if (c.variant != 0) return idb_fail(h, IDB_ERR_ARG, "idb_encode_condition: SMPL model only");
-    cudaStream_t st = (cudaStream_t)stream;
+    const int M = B * Tp, F = c.d_ff, H = c.n_heads, N = c.n_queries;
     const bool fused = h->gemm_backend == 1 && h->fused_mlp && idb_mlp_wgmma_supported(D, F);
-    if (M > d.enc_cap) {
-        for (void* p : d.enc_owned) cudaFree(p);
-        d.enc_owned.clear();
-        d.enc_cap = 0;
-        auto A = [&](float** p, size_t n) { if (cudaMalloc((void**)p, n * sizeof(float)) != cudaSuccess) return 1; d.enc_owned.push_back(*p); return 0; };
-        auto AH = [&](__half** p, size_t n) { if (cudaMalloc((void**)p, n * sizeof(__half)) != cudaSuccess) return 1; d.enc_owned.push_back(*p); return 0; };
-        int rc = 0;
-        rc |= A(&d.e_add, (size_t)M * D); rc |= A(&d.e_h, (size_t)M * D); rc |= A(&d.e_h2, (size_t)M * D); rc |= A(&d.e_z, (size_t)M * D);
-        rc |= A(&d.e_qkv, (size_t)M * (2 * D + H * D));
-        rc |= AH(&d.e_xtok_b, (size_t)M * Cp); rc |= AH(&d.e_xtok_s, (size_t)M * Cp);
-        rc |= AH(&d.e_h_b, (size_t)M * D); rc |= AH(&d.e_h_s, (size_t)M * D); rc |= AH(&d.e_h2_b, (size_t)M * D); rc |= AH(&d.e_h2_s, (size_t)M * D);
-        rc |= AH(&d.e_ff_b, (size_t)M * F); rc |= AH(&d.e_ff_s, (size_t)M * F);
-        if (rc) return idb_fail(h, IDB_ERR_CUDA, "out of device memory (encoder workspace)");
-        d.enc_cap = M;
-    }
     const bool pdl = h->pdl != 0;
     int rc;
-    k_cond_tokens<<<B, 256, 0, st>>>(past, pc_embedding, d.b_in, d.pe, d.e_xtok_b, d.e_xtok_s, d.e_add, C, Cp, Tp);
-    LAUNCH_CHECK(h);
     if ((rc = linear(h, d.e_xtok_b, d.e_xtok_s, Cp, d.w_in_b, d.w_in_s, Cp, nullptr, d.e_add, d.e_h, d.e_h_b, d.e_h_s, D, M, D, Cp, EPI_RES, st)))
         return rc;
     const dim3 slab_grid(B, (Tp + SLAB - 1) / SLAB);
@@ -1922,6 +1927,48 @@ extern "C" int idb_encode_condition(idb_handle* h, int B, int Tp, const float* p
                pending ? pending->ln3b : (const float*)nullptr, cond_out, B, Tp);
     LAUNCH_CHECK(h);
     return IDB_OK;
+}
+
+extern "C" int idb_encode_condition(idb_handle* h, int B, int Tp, const float* past, const float* pc_embedding, float* cond_out,
+                                    void* stream) {
+    IDB_ENTER(h);
+    if (!h || !past || !pc_embedding || !cond_out || B <= 0 || Tp <= 0) return IDB_ERR_ARG;
+    Denoiser& d = h->den;
+    if (!d.committed) return idb_fail(h, IDB_ERR_STATE, "idb_denoiser_commit first");
+    if (d.enc_layers.empty()) return idb_fail(h, IDB_ERR_STATE, "the conditioning encoder's weights (encoder.layers.*) were not loaded");
+    if (Tp > 36) return idb_fail(h, IDB_ERR_ARG, "supported past window: <= 36 frames");
+    const idb_denoiser_config& c = d.cfg;
+    const int C = c.c_body + c.c_obj, Cp = (C + 7) & ~7;
+    if (c.variant != 0) return idb_fail(h, IDB_ERR_ARG, "idb_encode_condition: SMPL model only");
+    cudaStream_t st = (cudaStream_t)stream;
+    int rc;
+    if ((rc = encoder_workspace(h, B * Tp, Cp))) return rc;
+    k_cond_tokens<<<B, 256, 0, st>>>(past, pc_embedding, d.b_in, d.pe, d.e_xtok_b, d.e_xtok_s, d.e_add, C, Cp, Tp);
+    LAUNCH_CHECK(h);
+    return encoder_layers(h, B, Tp, Cp, cond_out, st);
+}
+
+extern "C" int idb_encode_condition_skeleton(idb_handle* h, int B, int Tp, const float* body, const float* obj, const float* zero_pose_obj,
+                                             float* cond_out, void* stream) {
+    IDB_ENTER(h);
+    if (!h || !body || !obj || !zero_pose_obj || !cond_out || B <= 0 || Tp < 1) return IDB_ERR_ARG;
+    Denoiser& d = h->den;
+    if (!d.committed) return idb_fail(h, IDB_ERR_STATE, "idb_denoiser_commit first");
+    const idb_denoiser_config& c = d.cfg;
+    if (c.variant != 1) return idb_fail(h, IDB_ERR_ARG, "idb_encode_condition_skeleton: skeleton model only");
+    if (d.enc_layers.empty()) return idb_fail(h, IDB_ERR_STATE, "the conditioning encoder's weights (encoder.layers.*) were not loaded");
+    if (!d.shp_w) return idb_fail(h, IDB_ERR_STATE, "the object-shape embedding's weights (shapeEmbedding.*) were not loaded");
+    if (c.c_obj > IDB_SHAPE_EMB_MAX_IN) return idb_fail(h, IDB_ERR_STATE, "supported object keypoints: <= %d", IDB_SHAPE_EMB_MAX_IN / 3);
+    if (Tp > 36) return idb_fail(h, IDB_ERR_ARG, "supported past window: <= 36 frames");
+    // token rows share the input-embedding weight's padded width, which includes the decoder's 7 pose channels
+    const int Cp = (c.c_body + c.c_obj + c.c_extra + 7) & ~7;
+    cudaStream_t st = (cudaStream_t)stream;
+    int rc;
+    if ((rc = encoder_workspace(h, B * Tp, Cp))) return rc;
+    idb_cond_tokens_skeleton(body, obj, zero_pose_obj, d.shp_w, d.shp_b, d.b_in, d.pe, d.e_xtok_b, d.e_xtok_s, d.e_add, B, Tp, c.c_body,
+                             c.c_obj, Cp, st);
+    LAUNCH_CHECK(h);
+    return encoder_layers(h, B, Tp, Cp, cond_out, st);
 }
 
 extern "C" int idb_denoiser_forward(idb_handle* h, const float* x, const int64_t* timesteps, float* out, void* stream) {

@@ -298,6 +298,7 @@ class Engine:
         self._chk(self.lib.idb_denoiser_commit(self._h))
         self.variant = variant
         self.C = cfg.c_body + cfg.c_obj + cfg.c_extra
+        self.c_body, self.c_obj = cfg.c_body, cfg.c_obj
         self.D, self.n_heads, self.n_queries = D, n_heads, n_queries
 
     def bind(self, cond, T, zero_pose_obj=None):
@@ -433,6 +434,24 @@ class Engine:
         B, Tp = past.shape[0], past.shape[-1]
         out = torch.empty(Tp, B, 256, device=self.device)
         self._chk(self.lib.idb_encode_condition(self._h, B, Tp, self._ptr(past), self._ptr(pc), self._ptr(out), self._stream()))
+        return out
+
+    def encode_condition_skeleton(self, body, obj, zero_pose_obj, Tp):
+        """cond (Tp,B,256) of the skeleton model (reference model/diffusion_skeleton.py:194-215) from the first Tp frames of
+        body (T,B,n_joints,3) and obj (T,B,n_points,3), sequence-first, and zero_pose_obj (B,n_points,3); needs the
+        encoder.layers.* and shapeEmbedding.* weights loaded.  Non-contiguous inputs (e.g. a transposed batch) are copied."""
+        Tp = int(Tp)
+        if body.dim() != 4 or obj.dim() != 4 or not 1 <= Tp <= min(body.shape[0], obj.shape[0]):
+            raise EngineError("encode_condition_skeleton: body (T,B,J,3), obj (T,B,P,3) with 1 <= Tp <= T")
+        body, obj, zp = self._f32(body[:Tp]), self._f32(obj[:Tp]), self._f32(zero_pose_obj)
+        B = body.shape[1]
+        if (obj.shape[1], zp.shape[0]) != (B, B) or body[0, 0].numel() != self.c_body or obj[0, 0].numel() != self.c_obj \
+                or zp[0].numel() != self.c_obj:
+            raise EngineError("encode_condition_skeleton: shapes do not match the loaded model (%d body, %d object channels)"
+                              % (self.c_body, self.c_obj))
+        out = torch.empty(Tp, B, 256, device=self.device)
+        self._chk(self.lib.idb_encode_condition_skeleton(self._h, B, Tp, self._ptr(body), self._ptr(obj), self._ptr(zp), self._ptr(out),
+                                                         self._stream()))
         return out
 
     # ------------------------------------------------------------------ body model / geometry

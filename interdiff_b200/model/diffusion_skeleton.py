@@ -2,6 +2,7 @@
 :259-299): 21 body joints + 12 object keypoints + 7-D object pose (106 channels).  The object
 keypoints of the prediction are re-derived from the predicted pose inside the library
 (calc_obj_pred :218-229)."""
+import torch
 import torch.nn as nn
 
 from .diffusion_smpl import _EngineHost, _layer_stack, create_gaussian_diffusion  # noqa: F401
@@ -28,8 +29,18 @@ class MDM(_EngineHost, nn.Module):
         self.bodyFinalLinear = nn.Linear(D, args.smpl_dim)
         self.objFinalLinear = nn.Linear(D, 7)
 
+    def encode_condition(self, body, obj, zero_pose_obj, Tp):
+        """cond (Tp,B,D) from the first Tp frames of body (T,B,21,3), obj (T,B,12,3) and zero_pose_obj (B,12,3), on the
+        device (`idb_encode_condition_skeleton`)."""
+        return self.engine_for(body.device).encode_condition_skeleton(body, obj, zero_pose_obj, Tp)
+
     def _get_embeddings(self, body_gt, obj_gt, pose_gt, zero_pose_obj):
-        raise NotImplementedError("the conditioning encoder is the next row of the hot-path table (SURVEY.md 8f)")
+        """Reference :194-215: (embedding (Tp,B,D), gt (T,B,106)) from body_gt (T,B,21,3), obj_gt (T,B,12,3), pose_gt (T,B,7)
+        and zero_pose_obj (B,12,3), Tp = min(past_len, T) like the reference's slice."""
+        T, B = body_gt.shape[:2]
+        embedding = self.encode_condition(body_gt, obj_gt, zero_pose_obj, min(self.args.past_len, T))
+        gt = torch.cat([body_gt.reshape(T, B, -1), obj_gt.reshape(T, B, -1), pose_gt], dim=2)
+        return embedding, gt
 
     def forward(self, x, timesteps, zero_pose_obj, y=None):
         """x (B,1,106,T); zero_pose_obj (B,12,3) (reference :250-257)."""
